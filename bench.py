@@ -1,18 +1,19 @@
 #!/usr/bin/env python
-"""bench.py — fn evals/sec of compiled `pytensor.function(..., mode="CUDA")` graphs on B200, with parity, roofline and the
+"""bench.py — fn evals/sec of compiled `pytensor.function(..., mode="CUDA")` graphs on H100, with parity, roofline and the
 reference C linker beside every number.
 
 Contract (DESIGN.md §7):
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--skip a,b,...]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--skip a,b,...] [--dump-outputs DIR]
 
   N = 1 (plain `python bench.py`): headline = BASELINE.json configs[1] (cfg2, the 32-scalar-op fused Elemwise+CAReduce graph
       over fp32 (4096,4096)); a "step" is one evaluation of the compiled function.
-        value     evals/s, inputs resident in HBM, device outputs: MEDIAN over >= 25 windows of K steps each (CUDA events)
+        value     evals/s, inputs resident in HBM, device outputs: MEDIAN over the --reps windows that K timed steps are
+                  split into (CUDA events)
         e2e       evals/s through `pytensor.function(..., mode="CUDA")` with pinned HOST inputs and NumPy outputs
-        roofline  achieved HBM GB/s of the dominant kernel over MEASURED_PEAKS.json
+        roofline  achieved HBM GB/s of the dominant kernel over the H100 SXM data-sheet peak
         parity    CUDA outputs vs the reference C linker's outputs on the SAME 4096^2 arrays
       and, always on: `metric_graph` (the 265-node Elemwise+Gemm+Scan graph BASELINE.json's metric names, n=64 and
-      n=4096, with the C linker beside it), `cfg3` (MLP 4096^3: tcgen05 bf16 and the fp32-accurate default mode),
+      n=4096, with the C linker beside it), `cfg3` (MLP 4096^3: bf16 tensor cores and the fp32-accurate default mode),
       `cfg4` (Scan T=1000), `sharded_logp` (cfg5 on one GPU) — each with parity at the benchmarked shape.
   N > 1 (torchrun): headline = BASELINE.json configs[4] (cfg5): hierarchical logp+grad over world x 2^17 independent
       chains sharded along the batch axis, ONE all-reduce of the packed [logp, grads] (75 floats) per evaluation, issued
@@ -20,7 +21,11 @@ Contract (DESIGN.md §7):
       also carries the 1-GPU base measured in the same run, a strong-scaling point (2^20 chains in total), parity of
       the collective against a host sum of the per-rank partials and of rank 0's partial against the C linker, the
       N-rank collective self-test, and cfg2 replicas under `others`.
+  --steps K: the number of timed steps of the headline on every path (each `sharded_logp` measurement of N > 1 as well),
+      split into at most --reps windows; default 1250, and 50 host evaluations with --impl reference.
   --impl reference: the reference's own C linker (mode="CVM") on the host cores, same config strings (rank 0 only).
+  --dump-outputs DIR: after the timed steps, the headline workload's outputs of its last timed step (e, r) as DIR/<name>.npy;
+      the inputs are seeded, so two builds can be compared output for output.
 """
 
 from __future__ import annotations
@@ -44,36 +49,9 @@ N_ROWS, N_GROUPS, N_COV = 1024, 64, 8
 
 
 def _peaks():
-    p = os.path.join(REPO, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return {"hbm_gbs": d.get("hbm_gbs", 6650.0), "bf16_tflops": d.get("bf16_tflops", 1590.0),
-                "bf16_tflops_sustained": d.get("bf16_tflops_sustained", 1400.0), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
-
-
-def _ncu_traffic(kernel_prefix, pattern=("*prof_k3_final*_ncu_summary.csv", "*prof_ew*_ncu_summary.csv")):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed `ncu --set full`
-    capture summary of the same command (profiles/; the newest round's capture first); None when no capture is committed."""
-    import csv
-    import glob
-
-    patterns = (pattern,) if isinstance(pattern, str) else tuple(pattern)
-    paths = [p for pat in patterns for p in sorted(glob.glob(os.path.join(REPO, "profiles", pat)), reverse=True)]
-    for path in paths:
-        try:
-            rows = list(csv.reader(open(path)))
-            hdr, units = rows[0], rows[1]
-            kn, rd, wr = hdr.index("Kernel Name"), hdr.index("dram__bytes_read.sum"), hdr.index("dram__bytes_write.sum")
-            scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-            vals = [float(r[rd]) * scale.get(units[rd], 1.0) + float(r[wr]) * scale.get(units[wr], 1.0)
-                    for r in rows[2:] if r[kn].startswith(kernel_prefix) and not r[kn].endswith("_fin")]
-            if vals:
-                return sum(vals) / len(vals)
-        except Exception:  # noqa: BLE001
-            continue
-    return None
+    """NVIDIA's H100 SXM data-sheet figures (dense BF16, HBM3), for a card allowed 700 W: the denominators of the
+    `frac` fields, not rates this benchmark has reached.  The card's name and power limit are in `clocks`."""
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "H100 SXM data sheet"}
 
 
 def workload_config(world):
@@ -81,7 +59,7 @@ def workload_config(world):
     if world == 1:
         return {"workload": "cfg2 (BASELINE.json configs[1]): 32-scalar-op fused Elemwise+CAReduce graph, fp32 "
                             "(4096,4096) -> e (4096,4096) f32, r=e.sum(1) f32 (acc f64)",
-                "l2": "two alternating input sets, 384 MiB working set > 126 MB L2",
+                "l2": "two alternating input sets, 384 MiB working set > 50 MB L2",
                 "parallelism": "1 GPU"}
     return {"workload": "cfg5 (BASELINE.json configs[4]): hierarchical-normal logp+grad, n=1024 data rows, J=64 groups, "
                         f"K=8 covariates, batch = {world} x 2^17 independent chains (fp32), outputs summed over the batch",
@@ -90,10 +68,10 @@ def workload_config(world):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit")
 
     def __init__(self, index):
         self.index = index
@@ -131,8 +109,10 @@ class ClockSampler:
         mx = max(float(s[1]) for s in self.samples if s[1].replace(".", "").isdigit())
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for k, n in enumerate(names) if any(s[3 + k].lower().startswith("active") for s in self.samples)]
+        last = self.samples[-1]
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": reasons,
-                "samples": len(self.samples)}
+                "samples": len(self.samples), "gpu": last[7] if len(last) > 7 else None,
+                "power_limit_w": last[8] if len(last) > 8 else None}
 
 
 def pinned_like(arr):
@@ -197,22 +177,45 @@ def parity(got, exp, rtol=1e-5, atol=1e-5, note=None):
     return out
 
 
-def timed_windows(fn, steps, reps, sync, barrier=None):
-    """`reps` windows of `steps` calls each, CUDA events on the VM stream; returns per-window ms/step."""
+def timed_windows(fn, steps, reps, sync, barrier=None, total=None):
+    """`reps` windows of `steps` calls each, CUDA events on the VM stream; returns per-window ms/step.
+    With `total`, exactly `total` calls are timed, split into min(reps, total) windows whose sizes differ by at most one."""
     import torch
 
+    if total is not None:
+        w = max(1, min(reps, total))
+        sizes = [total // w + (1 if k < total % w else 0) for k in range(w)]
+    else:
+        sizes = [steps] * reps
     out = []
-    for _ in range(reps):
+    for n in sizes:
         if barrier is not None:
             barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        for i in range(steps):
+        for i in range(n):
             fn(i)
         e1.record()
         sync()
-        out.append(e0.elapsed_time(e1) / steps)
+        out.append(e0.elapsed_time(e1) / n)
     return out
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(dirname, named):
+    """Write each (name, host array) as <dirname>/<name>.npy in float32 / float64.  An array larger than its share of
+    DUMP_BYTES is replaced by every k-th row (a fixed sample, named <name>_rows_step<k>)."""
+    os.makedirs(dirname, exist_ok=True)
+    share = DUMP_BYTES // max(1, len(named))
+    for name, a in named:
+        a = np.asarray(a)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        if a.nbytes > share and a.ndim >= 1:
+            k = -(-a.nbytes // share)
+            a, name = a[::k], f"{name}_rows_step{k}"
+        np.save(os.path.join(dirname, name + ".npy"), np.ascontiguousarray(a))
 
 
 def window_stats(ms):
@@ -272,7 +275,7 @@ def _time_dev(f, dev_args, torch, steps, warm, reps=5):
 
 
 def bench_cfg3(pytensor, W, cuda_mode, dev, torch, peaks, cvm):
-    """configs[2]: 3-layer MLP 4096^3. bf16 tcgen05 mode and the default (fp32-accurate) mode, parity vs the C linker."""
+    """configs[2]: 3-layer MLP 4096^3. bf16 tensor-core mode and the default (fp32-accurate) mode, parity vs the C linker."""
     out = {}
     ins, outs, make_args, meta = W.cfg3_mlp(4096)
     host = make_args()
@@ -282,7 +285,7 @@ def bench_cfg3(pytensor, W, cuda_mode, dev, torch, peaks, cvm):
     exp = f_ref(*host)
     f_ref(*host)
     cpu_s = (time.perf_counter() - t0) / 2
-    for key, kw, steps, tol in (("bf16_tcgen05", {"gemm_precision": "bf16"}, 10, (2e-2, 2e-2)),
+    for key, kw, steps, tol in (("bf16_tc", {"gemm_precision": "bf16"}, 10, (2e-2, 2e-2)),
                                 ("default_fp32", {}, 3, (1e-5, 1e-5))):
         f = pytensor.function(ins, outs, mode=cuda_mode(device_outputs=True, borrow_outputs=True, **kw), trust_input=True)
         ms, st = _time_dev(f, a, torch, steps, 4)
@@ -465,6 +468,7 @@ def build_cfg5(pytensor, W, cuda_mode, B):
 
 
 def time_sharded(sh, argsets, steps, reps, torch, dist, warm=6):
+    """`steps` timed calls in total, split into at most `reps` windows; returns per-window ms/step."""
     for i in range(warm):
         res = sh(*argsets[i % len(argsets)], presharded=True)
 
@@ -474,7 +478,8 @@ def time_sharded(sh, argsets, steps, reps, torch, dist, warm=6):
         torch.cuda.synchronize()
 
     barrier()
-    ms = timed_windows(lambda i: sh(*argsets[i % len(argsets)], presharded=True), steps, reps, torch.cuda.synchronize, barrier)
+    ms = timed_windows(lambda i: sh(*argsets[i % len(argsets)], presharded=True), None, reps, torch.cuda.synchronize, barrier,
+                       total=steps)
     if dist is not None:
         t = torch.tensor(ms, device="cuda", dtype=torch.float64)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)  # per window: the slowest rank
@@ -580,7 +585,7 @@ def bench_cfg2(args, pytensor, W, cuda_mode, dev, jit, torch, dist, world, rank,
     f_dev = pytensor.function(ins, outs, mode=cuda_mode(device_outputs=True, borrow_outputs=True), trust_input=True)
     f_host = pytensor.function(ins, outs, mode="CUDA", trust_input=True)
     host_args = [make_args(1 + 10 * rank), make_args(101 + 10 * rank)]
-    dev_args = [[dev.to_device(a) for a in s] for s in host_args]  # two input sets: 2 x 128 MiB > the 126 MB L2
+    dev_args = [[dev.to_device(a) for a in s] for s in host_args]  # two input sets: 2 x 128 MiB > the 50 MB L2
 
     def barrier():
         if dist is not None:
@@ -598,7 +603,15 @@ def bench_cfg2(args, pytensor, W, cuda_mode, dev, jit, torch, dist, world, rank,
             for i in range(16):
                 f_dev(*dev_args[i % 2])
             torch.cuda.synchronize()
-        ms_w = timed_windows(lambda i: f_dev(*dev_args[i % 2]), args.steps, reps, torch.cuda.synchronize, barrier)
+        last = {}
+
+        def step(i):
+            last["out"], last["i"] = f_dev(*dev_args[i % 2]), i
+
+        ms_w = timed_windows(step, None, reps, torch.cuda.synchronize, barrier, total=args.steps)
+        if args.dump_outputs and rank == 0:
+            # the timed path's device outputs of its last step, before any further call reuses their buffers
+            dump_outputs(args.dump_outputs, list(zip(("e", "r"), (dev.to_host(o) for o in last["out"]))))
         t_end = time.perf_counter() + 0.6
         while time.perf_counter() < t_end:  # keep the same load up so that later nvidia-smi samples see it
             for i in range(64):
@@ -664,13 +677,13 @@ def bench_cfg2(args, pytensor, W, cuda_mode, dev, jit, torch, dist, world, rank,
     alg_bytes = meta["bytes"] if fused else 3 * 4 * args.n * args.n
     # duration of the dominant kernel: when a step IS one launch of it (the fused graph: a CUDA graph with that single
     # kernel node), its average duration over the timed region is the region's time per step — CUDA events around
-    # K x reps launches, no per-launch event overhead; the per-launch event pair of the eager profile run (which
-    # over-reads a ~40 us kernel by ~3 us) is reported beside it
+    # the K timed launches, no per-launch event overhead; the per-launch event pair of the eager profile run (which
+    # includes the event overhead) is reported beside it
     one_launch = launches_per_step == 1 and replayed
     kernel_ms = ms if one_launch else step_ms[dom]
     achieved = alg_bytes / (kernel_ms * 1e-3) / 1e9
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                "frac": achieved / peaks["hbm_gbs"], "traffic": _ncu_traffic("ptk_ew_red_row" if fused else "ptk_ew_vec"),
+                "frac": achieved / peaks["hbm_gbs"],
                 "kernel": dom_name, "kernel_ms": kernel_ms, "algorithmic_bytes": alg_bytes, "peak_source": peaks["source"],
                 "launches_per_step": launches_per_step,
                 "how": ("one launch of this kernel per step: kernel_ms = CUDA-event time of the timed region / launches "
@@ -700,7 +713,7 @@ def bench_cfg2(args, pytensor, W, cuda_mode, dev, jit, torch, dist, world, rank,
                    "steps": e2e_steps, "windows": 5,
                    "pipeline": ("chunked H2D|kernel|D2H x%d" % len(f_host.vm.executor._chunk_plan["bounds"]))
                    if f_host.vm.executor.chunked_calls else "one-shot"},
-           "gpu_launches": launches_per_step * args.steps * reps, "roofline": roofline, "cpu_baseline": cpu, "parity": par,
+           "gpu_launches": launches_per_step * args.steps, "roofline": roofline, "cpu_baseline": cpu, "parity": par,
            "clocks": clocks.summary()}
     return rec
 
@@ -725,14 +738,22 @@ def bench_k1_stream(pytensor, cuda_mode, dev, torch, peaks):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--steps", type=int, default=None,
+                    help="timed steps of the headline workload, split into --reps windows (default 1250; "
+                         "--impl reference: 50 evaluations on the host)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--n", type=int, default=4096)
-    ap.add_argument("--reps", type=int, default=25, help="timed windows of --steps steps each (median reported)")
+    ap.add_argument("--reps", type=int, default=25, help="timed windows (median reported)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline workload's outputs of its last timed step as DIR/<name>.npy (at most 64 MB)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--skip", default="", help="comma list of: metric,cfg3,cfg4,cfg5,k1,cfg2 (developer runs)")
     args = ap.parse_args()
+    if args.steps is None:
+        args.steps = 50 if args.impl == "reference" else 1250
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     skip = {s for s in args.skip.split(",") if s}
     rank = int(os.environ.get("RANK", "0"))
@@ -776,7 +797,7 @@ def main():
 
     base = {"metric": "fn evals/sec", "unit": "evals/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
-            "config": workload_config(world), "timing": {"windows": reps, "steps_per_window": args.steps,
+            "config": workload_config(world), "timing": {"windows": min(reps, max(1, args.steps)), "timed_steps": args.steps,
                                                          "statistic": "median over windows (per window: max over ranks)"}}
 
     if world == 1:
@@ -795,7 +816,7 @@ def main():
             line["cfg4"] = guarded(bench_cfg4, pytensor, W, cuda_mode, dev, torch, peaks, cvm)
         if "cfg5" not in skip:
             def one_gpu_cfg5():
-                rec, f, sh, local, host_sets = sharded_logp(pytensor, W, cuda_mode, dev, torch, None, 1, 0, 20, 9, "none",
+                rec, f, sh, local, host_sets = sharded_logp(pytensor, W, cuda_mode, dev, torch, None, 1, 0, 180, 9, "none",
                                                             check=True, cvm=cvm if want_cpu else None)
                 f_host = pytensor.function(*cfg5_io(W, B_LOCAL), mode="CUDA", trust_input=True)
                 s, h2d, d2h = e2e_cfg5(f_host, host_sets, 10, 5, torch, None)
@@ -824,12 +845,12 @@ def main():
     line.update({"value": world * 1e3 / med, "ms_per_step": med, "windows": rec["windows"], "clocks": clocks.summary(),
                  "parity": rec.pop("parity", None), "collective_selftest": selftest, "weak_scaling_base_1gpu": base1})
     launches = len(f.vm.executor.program.steps)
-    line["gpu_launches"] = launches * args.steps * reps
+    line["gpu_launches"] = launches * args.steps
     alg = sum(a.nbytes for a in host_sets[0]) + 4 * 75
     dom_ms = guarded(lambda: dominant_kernel_ms(f, local[0], dev, torch))
     if isinstance(dom_ms, tuple):
         line["roofline"] = {"bound": "hbm", "achieved": alg / (dom_ms[1] * 1e-3) / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                            "frac": alg / (dom_ms[1] * 1e-3) / 1e9 / peaks["hbm_gbs"], "traffic": _ncu_traffic("ptk_rowfuse", "*cfg5*_ncu_summary.csv"),
+                            "frac": alg / (dom_ms[1] * 1e-3) / 1e9 / peaks["hbm_gbs"],
                             "kernel": dom_ms[0], "kernel_ms": dom_ms[1], "algorithmic_bytes": alg, "peak_source": peaks["source"],
                             "note": "the fused likelihood kernel reads every parameter once (B x 74 floats) and does ~46 flop "
                                     "per (chain, data row): it is fp32-issue-bound, not HBM-bound — see DESIGN.md §4"}

@@ -1,5 +1,5 @@
 /*
- * ptk.h — C-ABI of libptk.so, the B200 (sm_100a) kernel library behind pytensor.link.cuda.CUDALinker.
+ * ptk.h — C-ABI of libptk.so, the H100 (sm_90a) kernel library behind pytensor.link.cuda.CUDALinker.
  *
  * Conventions (mirrors the reference's C-thunk ABI: `int (*fn)(void* data)` returning 0 on success and stashing
  * the error beside it — /root/reference/pytensor/link/c/c_code/lazylinker_c.c:498-534, link/c/basic.py:1690-1761):
@@ -52,7 +52,7 @@ ptk_status   ptk_host_free_pinned(void* p);
 
 /* ---- JIT: the per-Composite kernels (replaces the per-node g++ compile of the C linker:
  *      pytensor/link/c/cmodule.py:2454-2643 GCC_compiler.compile_str, link/c/basic.py:1585 cthunk_factory) -------- */
-/* Compile CUDA C++ `src` for sm_100a with NVRTC. On success *cubin / *cubin_size receive a malloc'd image the caller
+/* Compile CUDA C++ `src` for sm_90a with NVRTC. On success *cubin / *cubin_size receive a malloc'd image the caller
  * releases with ptk_free(). `log` (may be NULL) receives a malloc'd compile log (also on failure). */
 ptk_status   ptk_jit_compile(const char* src, const char* const* opts, int n_opts,
                              void** cubin, size_t* cubin_size, char** log);
@@ -151,8 +151,8 @@ ptk_status   ptk_random_fill(int dist, int dtype, void* out, int64_t n, uint64_t
  *      Ger tensor/blas/ger.py:8; the C linker calls sgemm_/dgemm_/sgemv_/dgemv_ at blas/c_code/codegen.py:463-805) */
 /* C[M,N] = alpha * A[M,K] @ B[K,N] + beta * C, arbitrary element strides, dtype PTK_F32 | PTK_F64.
  * beta == 0 never reads C (so an AllocEmpty C holding NaNs is fine — gemv.py:79-86 contract).
- * precision: 0 = native (fp32/fp64 FMA, <=1e-5 rel vs BLAS), 1 = bf16 operands on tcgen05 tensor cores with fp32
- * TMEM accumulation (fp32 graphs only; needs `workspace` of ptk_gemm_workspace_bytes()). */
+ * precision: 0 = native (fp32/fp64 FMA, <=1e-5 rel vs BLAS), 1 = bf16 operands on wgmma tensor cores with fp32
+ * accumulation (fp32 graphs only; needs `workspace` of ptk_gemm_workspace_bytes()). */
 size_t       ptk_gemm_workspace_bytes(int64_t M, int64_t N, int64_t K, int precision);
 ptk_status   ptk_gemm(int dtype, int64_t M, int64_t N, int64_t K, double alpha,
                       const void* A, int64_t sa0, int64_t sa1, const void* B, int64_t sb0, int64_t sb1,
@@ -163,13 +163,12 @@ ptk_status   ptk_gemm_bias_act(int dtype, int64_t M, int64_t N, int64_t K,
                       const void* A, int64_t sa0, int64_t sa1, const void* B, int64_t sb0, int64_t sb1,
                       const void* bias, int act, void* C, int64_t sc0, int64_t sc1,
                       int precision, void* workspace, size_t workspace_bytes, void* stream);
-/* Extended tensor-core entry point (fp32 graphs, bf16 operands, fp32 TMEM accumulation):
+/* Extended tensor-core entry point (fp32 graphs, bf16 operands, fp32 accumulation):
  *   C = act(alpha * A @ B + beta * C + bias[N]);
  * A comes either as fp32 (A_f32, element strides sa0/sa1; staged to bf16 in the workspace) or ALREADY staged as bf16
  * (A_bf16: row-major [M,K], pitch lda_bf16 elements (multiple of 8), 16-byte aligned) — e.g. the C_bf16 copy a previous
  * call emitted, so that a chain of layers re-stages only the weights.  C_bf16 (optional, row-major pitch ldc_bf16) receives
- * a bf16 copy of the result.  Environment PTK_GEMM_MODE selects the kernel: 1 = single CTA per tile,
- * 2 = 2-CTA cluster sharing the B tile by TMA multicast, 3 = cta_group::2 UMMA (one 256x256 tile per CTA pair). */
+ * a bf16 copy of the result. */
 ptk_status   ptk_gemm_tc_ex(int64_t M, int64_t N, int64_t K, double alpha, const void* A_f32, int64_t sa0, int64_t sa1,
                       const void* A_bf16, int64_t lda_bf16, const void* B_f32, int64_t sb0, int64_t sb1, double beta,
                       void* C, int64_t sc0, int64_t sc1, const void* bias, int act, void* C_bf16, int64_t ldc_bf16,
@@ -178,7 +177,7 @@ ptk_status   ptk_gemm_tc_ex(int64_t M, int64_t N, int64_t K, double alpha, const
  * here: pytensor/tensor/blas/c_code/codegen.py:463-540; parity bar <= 1e-5 vs that result):
  *   C = act(alpha * A @ B + beta * C + bias[N]),  A, B, C fp32 with arbitrary element strides.
  * Each operand is staged as THREE bf16 pieces x = x1 + x2 + x3 (24 mantissa bits in total); per 64-wide k-block the
- * cta_group::2 tcgen05 kernel accumulates `terms` piece products in the fp32 TMEM accumulator, smallest first:
+ * wgmma kernel accumulates `terms` piece products in its fp32 register accumulator, smallest first:
  *   terms = 6: A3B1+A2B2+A1B3+A2B1+A1B2+A1B1 (only O(2^-24) products dropped: below sgemm's own rounding noise),
  *   terms = 3: A2B1+A1B2+A1B1 (about 4e-6 of the output scale at K = 4096; twice as fast).
  * workspace >= ptk_gemm_split_workspace_bytes(M, N, K), caller-owned. */
@@ -201,7 +200,7 @@ ptk_status   ptk_gemm_tc_split(int64_t M, int64_t N, int64_t K, double alpha, co
  *     operand layout ptk_gemm_tc_staged's exact_main mode expects for both A and B.
  *   ptk_gemm_tc_staged: C = act(alpha * A @ B + beta * C + bias[N]) from staged A [M,K] / B^T [N,K]; terms 1 (bf16
  *     operands) | 3 | 6 (fp32-accurate, see ptk_gemm_tc_split; 3 and 6 need 3-piece operands).  exact_main != 0 (both
- *     operands staged `aligned`): A1 x B1 accumulates in its own TMEM accumulator — exactly while its partial sums stay below
+ *     operands staged `aligned`): A1 x B1 accumulates in its own accumulator — exactly while its partial sums stay below
  *     2^24 units (always for K <= 1024; see ptk_gemm_tc.cu lead_bits_for), in chunks only beyond K = 16384; the
  *     correction products in a second one; the epilogue adds them with round-to-nearest.  C_stage (optional) receives
  *     out_pieces (1 | 3) staged pieces of the result [M,N] (pitch ldc_stage, piece pitch c_rows); out_exp != PTK_STAGE_NO_EXP

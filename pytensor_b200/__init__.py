@@ -1,4 +1,4 @@
-"""pytensor_b200 — a B200-native (sm_100a) graph-execution backend for PyTensor.
+"""pytensor_b200 — an H100-native (sm_90a) graph-execution backend for PyTensor.
 
     import pytensor_b200            # registers mode="CUDA" / "CUDA_BF16" with the host PyTensor
     f = pytensor.function([x], y, mode="CUDA")

@@ -515,7 +515,20 @@ def gen_region_kernel(plan: RegionPlan, dims: dict, ext: list, name: str, idx_ch
                     L.pre.append(f"for (int jj = lane; jj < {nb}; jj += 32) sm{buf}[jj] = 0;")
                     L.pre.append("__syncwarp();")
                     ix = index_expr(L, idx, nb)
-                    L.body.append(f"atomicAdd(&sm{buf}[{ix}], {L.pt(y)});")
+                    if vals[buf].dtype == "float64":
+                        # fp64 shared-memory atomicAdd is a compare-and-swap loop on sm_90, so lanes that hit the same
+                        # bin would add in an arbitrary order; adding in lane order (the lanes of one iteration are
+                        # consecutive positions j) keeps the sum bit-equal to a sequential scatter-add
+                        L.body.append("#ifdef __CUDA_ARCH__")
+                        L.body.append(f"{{ const int pix = {ix}; const double pv = {L.pt(y)};"
+                                      f" const unsigned pm = ({n} - (j - lane) >= 32) ? 0xffffffffu"
+                                      f" : ((1u << ({n} - (j - lane))) - 1u);"
+                                      f" for (int q = 0; q < 32; ++q) {{ if (lane == q) sm{buf}[pix] += pv; __syncwarp(pm); }} }}")
+                        L.body.append("#else")
+                        L.body.append(f"atomicAdd(&sm{buf}[{ix}], {L.pt(y)});")
+                        L.body.append("#endif")
+                    else:
+                        L.body.append(f"atomicAdd(&sm{buf}[{ix}], {L.pt(y)});")
                     L.writes_smem = True
                 elif m.kind == "put_fin":
                     x = op.ins[0]

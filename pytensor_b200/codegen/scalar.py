@@ -555,7 +555,7 @@ def emit_body(prog: ScalarProgram, fn_name: str = "ptk_body") -> str:
     for k, inst in enumerate(prog.insts):
         fn = OPS.get(inst.op)
         if fn is None:
-            raise UnsupportedScalarOp(f"scalar op {inst.op} has no sm_100a device expression yet")
+            raise UnsupportedScalarOp(f"scalar op {inst.op} has no sm_90a device expression yet")
         args = [_ref_expr(r, prog) for r in inst.args]
         expr = fn(args, inst.in_dtypes, inst.out_dtype)
         T = CTYPE[inst.out_dtype]

@@ -1,11 +1,11 @@
-// bf16 tensor-core GEMM for fp32 graphs on sm_100a: tcgen05.mma (cta_group::1, M=128, N=256, K=16) with fp32
-// accumulators in TMEM, operands staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) through a 4-stage mbarrier ring,
-// persistent CTAs (one per SM) with a double-buffered TMEM accumulator so that the epilogue of tile i overlaps the MMAs
-// of tile i+1.  Warp roles: warp 0 = TMA producer, warp 1 = MMA issuer (one elected lane), warp 2 = TMEM allocator,
-// warps 4-7 = epilogue (tcgen05.ld 32x32b -> alpha/beta/bias/tanh -> global).
+// bf16 tensor-core GEMM for fp32 graphs on sm_90a (H100): warpgroup MMA (wgmma.mma_async m64n128k16, bf16 x bf16 ->
+// fp32 accumulators in registers), operands staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) through a 6-stage
+// mbarrier ring.  One CTA per 128 x 128 output tile, three warpgroups: warpgroup 0 = TMA producer (one thread),
+// warpgroups 1 and 2 = consumers, each owning 64 rows of the tile: they issue the wgmmas and run the epilogue
+// (alpha/beta/bias/tanh -> global) straight from their accumulator registers.
 //
 // Replaces the sgemm_ call the C linker emits for Dot22 / Gemm (pytensor/tensor/blas/c_code/codegen.py:463-540) on the
-// "bf16 on tcgen05" configuration of BASELINE.json: the graph dtype stays float32 (the reference has no bfloat16 dtype,
+// "bf16 tensor core" configuration of BASELINE.json: the graph dtype stays float32 (the reference has no bfloat16 dtype,
 // pytensor/tensor/type.py:40-55), operands are rounded to bf16 by a conversion pass into a caller-owned workspace
 // (A as [M,K] K-major, B transposed to [N,K] K-major), products accumulate in fp32.
 #include <cuda_bf16.h>
@@ -16,17 +16,16 @@
 namespace {
 
 constexpr int BLOCK_M = 128;
-constexpr int BLOCK_N = 256;
+constexpr int BLOCK_N = 128;
 constexpr int BLOCK_K = 64;   // 64 bf16 = 128 bytes = one SWIZZLE_128B row
-constexpr int UMMA_K = 16;
-constexpr int STAGES = 4;
-constexpr int ACC_STAGES = 2;
-constexpr int TMEM_COLS = 512;  // 2 accumulators x 256 fp32 columns
-constexpr int NUM_THREADS = 256;
+constexpr int WG_K = 16;      // K of one wgmma
+constexpr int STAGES = 6;
+constexpr int NUM_THREADS = 384;
 constexpr uint32_t A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KiB
-constexpr uint32_t B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;  // 32 KiB
+constexpr uint32_t B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;  // 16 KiB
 constexpr uint32_t STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
 constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+static_assert(SMEM_BYTES <= 227 * 1024, "H100 allows at most 227 KiB of shared memory per block");
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -58,9 +57,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int32_t c0, int32_t c1) {
   asm volatile(
@@ -69,86 +65,68 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_mc(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int32_t c0, int32_t c1,
-                                               uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], "
-      "[%2], %5;" ::"r"(smem_u32(smem_dst)),
-      "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// Ties the accumulator registers to the surrounding asm statements: the compiler may neither read them before the
+// wgmma.wait_group that completes them nor move an epilogue write past the wgmma.fence that precedes the next MMA.
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int j = 0; j < N; ++j) asm volatile("" : "+f"(r[j])::"memory");
 }
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, bf16 x bf16 -> fp32
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+
+// D (+)= A[smem desc] * B[smem desc]^T for a 64 x 128 x 16 slice, bf16 x bf16 -> fp32, both operands K-major.
+// Accumulator fragment: thread t of the warpgroup holds rows 16 * (t / 32) + (t % 32) / 4 (+ 8) and columns
+// 8 * j + 2 * (t % 4) (+ 1): d[4j + 2h + e] = D[row + 8h][8j + 2(t % 4) + e].
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+      "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+      "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
+// K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 wgmma layout):
 //  [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused for swizzled K-major) |
-//  [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024 B between row groups) | [46,48) version = 1 |
-//  [61,64) layout type = 2 (SWIZZLE_128B)
+//  [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024 B between row groups) | [62,64) layout type = 1 (SWIZZLE_128B)
+// Stepping K by 16 inside the 128-byte swizzle row advances the start address by 32 bytes (the tile is 1024-aligned).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1) @4, a/b format BF16 (1) @7/@10, both K-major,
-// N>>3 @17, M>>4 @24.
-__host__ __device__ constexpr uint32_t make_idesc(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
 }
 
 struct EpiParams {
@@ -160,28 +138,24 @@ struct EpiParams {
   int M, N, K;
   __nv_bfloat16* Cbf;  // optional bf16 copy of the result, row-major [M, ldcbf] (the next layer's K-major A operand)
   long long ldcbf;
-  int out_pieces;      // pair kernel: 1 = Cbf is a plain bf16 copy; 3 = the three-piece split of the result (piece i at rows
+  int out_pieces;      // 1 = Cbf is a plain bf16 copy; 3 = the three-piece split of the result (piece i at rows
   long long cbf_rows;  // [i * cbf_rows, ...) of Cbf) — the staged A operand of a following fp32-accurate product
-  int split_tail;      // pair kernel: split the units of the last partial round into 256 x 128 halves (PTK_GEMM_SPLIT=0: off)
-  // fp32-accurate mode (pair kernel): every fp32 operand is staged as THREE bf16 pieces x = x1 + x2 + x3 (8 mantissa bits
-  // each) stacked along the rows of the staging matrix (piece i of A at rows [i * a_rows, ...)); per k-block the kernel
-  // accumulates `terms` piece products into the same fp32 TMEM accumulator, smallest first:
+  // fp32-accurate mode: every fp32 operand is staged as THREE bf16 pieces x = x1 + x2 + x3 (8 mantissa bits each) stacked
+  // along the rows of the staging matrix (piece i of A at rows [i * a_rows, ...)); per k-block the kernel accumulates
+  // `terms` piece products into the same fp32 accumulator, smallest first:
   //   terms = 6: A3B1 + A2B2 + A1B3 + A2B1 + A1B2 + A1B1   (drops only O(2^-24) terms: below sgemm's own rounding noise)
   //   terms = 3:                      A2B1 + A1B2 + A1B1   (~4e-6 of the output scale at K = 4096)
   //   terms = 1: plain bf16 operands (the CUDA_BF16 mode)
   int terms;
   int a_rows, b_rows;  // row pitch between the stacked pieces
-  // pair kernel: k-blocks per ACCUMULATION CHUNK (0 = the whole K in one chunk).  The tensor core adds into its fp32
-  // accumulator with truncation, a bias that grows linearly with the length of the accumulation chain (measured: ~6e-9 x K
-  // of the output scale, 2.4e-5 at K = 4096 — more than the whole 1e-5 budget of the fp32-accurate mode).  With chunks the
-  // TMEM accumulator only ever holds the sum over `kchunk` k-blocks; the epilogue adds every chunk into C in global memory
-  // with round-to-nearest fp32 adds (the same thread owns the same elements for all chunks of a tile, so the
-  // read-modify-write needs no synchronisation) and applies bias / activation / the bf16 copy after the last chunk.
+  // k-blocks per ACCUMULATION CHUNK (0 = the whole K in one chunk).  The tensor core adds into its fp32 accumulator with
+  // truncation, a bias that grows linearly with the length of the accumulation chain.  With chunks the register
+  // accumulator only ever holds the sum over `kchunk` k-blocks; the epilogue adds every chunk into C in global memory with
+  // round-to-nearest fp32 adds (the same thread owns the same elements for all chunks of a tile, so the read-modify-write
+  // needs no synchronisation) and applies bias / activation / the bf16 copy after the last chunk.
   int kchunk;
-  // pair kernel, fp32-accurate mode with an error-free leading piece (see row_absmax_kernel): the A1 x B1 products go
-  // to the accumulator at TMEM columns [0, 256), the correction products to the one at [256, 512); the epilogue adds the
-  // two (round to nearest).  Both buffers form ONE accumulator stage, so the epilogue of a chunk does not overlap the
-  // next chunk's MMAs.
+  // fp32-accurate mode with an error-free leading piece (see row_absmax_kernel): the A1 x B1 products go to the main
+  // accumulator, the correction products to a second one; the epilogue adds the two (round to nearest).
   int exact_main;
   // staged output pieces (Cbf, out_pieces == 3): leading piece aligned to the fixed exponent out_exp (operands known to lie
   // in [-1, 1]) so that it can feed an exact-main product; PTK_NO_EXP: ordinary bf16 split
@@ -193,560 +167,190 @@ struct EpiParams {
 __device__ __constant__ int kPieceA[6] = {2, 1, 0, 1, 0, 0};
 __device__ __constant__ int kPieceB[6] = {0, 1, 2, 0, 1, 0};
 
-// kCluster == 2: CTA pairs (cluster 2x1x1) share the B tile of a 256-row super-tile — each CTA loads HALF of it and
-// TMA-multicasts that half into both CTAs' shared memory, cutting the L2->SM traffic per CTA from 48 to 32 KiB per
-// k-block (the single-CTA kernel is L2-bandwidth bound: 1.6 GB per 4096^3 GEMM at ~12 TB/s).  A shared-memory stage
-// may be refilled only when BOTH CTAs' MMAs have drained it: the stage's "empty" barrier counts 2 arrivals and every
-// tcgen05.commit is multicast to the pair.
-template <int kCluster>
+// One output element pair (row, col), (row, col + 1) of a finished chunk: alpha * acc (+ beta * C) (+ bias) (tanh), the
+// bf16 / three-piece copy.  The vector and the scalar branch compute the same values.
+__device__ __forceinline__ void epi_pair(const EpiParams& p, long long row, long long col, float v0, float v1, float beta,
+                                         const float* bias, int act, __nv_bfloat16* cbf) {
+  if (row >= p.M || col >= p.N) return;
+  const bool two = col + 1 < p.N;
+  float* dst = p.C + row * p.sc0 + col * p.sc1;
+  const bool vec = two && p.sc1 == 1 && ((((uintptr_t)dst) & 7) == 0);
+  float x[2] = {p.alpha * v0, p.alpha * v1};
+  if (beta != 0.0f) {
+    if (vec) {
+      const float2 o = __ldcg(reinterpret_cast<const float2*>(dst));
+      x[0] += beta * o.x;
+      x[1] += beta * o.y;
+    } else {
+      x[0] += beta * dst[0];
+      if (two) x[1] += beta * dst[p.sc1];
+    }
+  }
+  if (bias) {
+    x[0] += bias[col];
+    if (two) x[1] += bias[col + 1];
+  }
+  if (act == 1) {
+    x[0] = tanhf(x[0]);
+    x[1] = tanhf(x[1]);
+  }
+  if (vec) {
+    *reinterpret_cast<float2*>(dst) = make_float2(x[0], x[1]);
+  } else {
+    dst[0] = x[0];
+    if (two) dst[p.sc1] = x[1];
+  }
+  if (cbf) {
+    for (int pc = 0; pc < p.out_pieces; ++pc) {   // piece pc = bf16 of what the earlier pieces left over
+      __nv_bfloat16 b[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        b[e] = (pc == 0 && p.out_exp != PTK_NO_EXP) ? __float2bfloat16_rn(rintf(x[e] * p.out_scale) * p.out_inv)
+                                                    : __float2bfloat16_rn(x[e]);
+        x[e] -= __bfloat162float(b[e]);
+      }
+      __nv_bfloat16* d = cbf + ((long long)pc * p.cbf_rows + row) * p.ldcbf + col;
+      if (two && ((((uintptr_t)d) & 3) == 0)) {
+        __nv_bfloat162 pk;
+        pk.x = b[0];
+        pk.y = b[1];
+        *reinterpret_cast<__nv_bfloat162*>(d) = pk;
+      } else {
+        d[0] = b[0];
+        if (two) d[1] = b[1];
+      }
+    }
+  }
+}
+
+// kExact: compile-time copy of EpiParams::exact_main — the plain instantiation carries no second accumulator.
+template <bool kExact>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_bf16_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, EpiParams p) {
+gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, EpiParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* smem_a = smem;                              // STAGES x 16 KiB
-  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;     // STAGES x 32 KiB
+  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;     // STAGES x 16 KiB
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* full_bar = bars;                    // [STAGES]
-  uint64_t* empty_bar = bars + STAGES;          // [STAGES]
-  uint64_t* tmem_full = bars + 2 * STAGES;      // [ACC_STAGES]
-  uint64_t* tmem_empty = bars + 2 * STAGES + ACC_STAGES;  // [ACC_STAGES]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 2 * ACC_STAGES);
+  uint64_t* full_bar = bars;                    // [STAGES]  TMA bytes landed
+  uint64_t* empty_bar = bars + STAGES;          // [STAGES]  8 arrivals: every consumer warp is done reading
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M, n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
-  const uint32_t crank = (kCluster > 1) ? cluster_ctarank() : 0u;
-  // work decomposition: a "unit" is kCluster vertically adjacent M-tiles of one N-tile; units are dealt round-robin
-  const int m_groups = (m_tiles + kCluster - 1) / kCluster;
-  const int num_units = m_groups * n_tiles;
-  const int unit0 = blockIdx.x / kCluster, unit_stride = gridDim.x / kCluster;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmap_a);
-    prefetch_tmap(&tmap_b);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kCluster);
-    }
-    for (int a = 0; a < ACC_STAGES; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 4);  // one arrive per epilogue warp
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc(tmem_ptr, TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  if (kCluster > 1) cluster_sync_all();  // the peer's barriers must be initialised before anything is multicast to them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ===== TMA producer =====
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int u = unit0; u < num_units; u += unit_stride) {
-        const int tm = (u % m_groups) * kCluster + (int)crank, tn = u / m_groups;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
-          tma_load_2d(&tmap_a, &full_bar[stage], smem_a + stage * A_STAGE_BYTES, kb * BLOCK_K, tm * BLOCK_M);
-          if (kCluster == 1) {
-            tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES, kb * BLOCK_K, tn * BLOCK_N);
-          } else {
-            constexpr uint32_t HALF = B_STAGE_BYTES / 2;  // 128 rows of the B tile
-            tma_load_2d_mc(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES + crank * HALF, kb * BLOCK_K,
-                           tn * BLOCK_N + (int)crank * (BLOCK_N / 2), (uint16_t)0x3);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer (single thread) =====
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(BLOCK_M, BLOCK_N);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int u = unit0; u < num_units; u += unit_stride) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);  // epilogue drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * BLOCK_N;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem_a + stage * A_STAGE_BYTES);
-          const uint32_t b_addr = smem_u32(smem_b + stage * B_STAGE_BYTES);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            const uint64_t a_desc = make_smem_desc(a_addr + k * UMMA_K * 2);
-            const uint64_t b_desc = make_smem_desc(b_addr + k * UMMA_K * 2);
-            umma_f16(d_tmem, a_desc, b_desc, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          // frees the smem slot once these MMAs have read it (in both CTAs of the pair when the B tile is shared)
-          if (kCluster == 1) umma_commit(&empty_bar[stage]);
-          else umma_commit_mc(&empty_bar[stage], (uint16_t)0x3);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator complete -> epilogue
-        if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: TMEM -> registers -> global =====
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int u = unit0; u < num_units; u += unit_stride) {
-      const int tm = (u % m_groups) * kCluster + (int)crank, tn = u / m_groups;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const long long row = (long long)tm * BLOCK_M + q * 32 + lane;
-      const bool row_ok = row < p.M;
-      float* crow = p.C + row * p.sc0;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BLOCK_N; c0 += 32) {
-        uint32_t r[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BLOCK_N + c0);
-        tmem_ld_32x32b_x32(taddr, r);
-        tmem_ld_wait();
-        const long long col0 = (long long)tn * BLOCK_N + c0;
-        if (row_ok && col0 < p.N) {
-          const bool full = (col0 + 32 <= p.N);
-          if (full && p.sc1 == 1 && p.beta == 0.0f && ((((uintptr_t)(crow + col0)) & 15) == 0)) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              float4 v;
-              float* vv = reinterpret_cast<float*>(&v);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float x = p.alpha * __uint_as_float(r[j + e]);
-                if (p.bias) x += p.bias[col0 + j + e];
-                if (p.act == 1) x = tanhf(x);
-                vv[e] = x;
-              }
-              *reinterpret_cast<float4*>(crow + col0 + j) = v;
-              if (p.Cbf) {
-                __nv_bfloat162 lo = __floats2bfloat162_rn(vv[0], vv[1]), hi = __floats2bfloat162_rn(vv[2], vv[3]);
-                uint2 pk;
-                pk.x = *reinterpret_cast<uint32_t*>(&lo);
-                pk.y = *reinterpret_cast<uint32_t*>(&hi);
-                *reinterpret_cast<uint2*>(p.Cbf + row * p.ldcbf + col0 + j) = pk;
-              }
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const long long col = col0 + j;
-              if (col < p.N) {
-                float* dst = crow + col * p.sc1;
-                float x = p.alpha * __uint_as_float(r[j]);
-                if (p.beta != 0.0f) x += p.beta * (*dst);
-                if (p.bias) x += p.bias[col];
-                if (p.act == 1) x = tanhf(x);
-                *dst = x;
-                if (p.Cbf) p.Cbf[row * p.ldcbf + col] = __float2bfloat16_rn(x);
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == ACC_STAGES) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (kCluster > 1) cluster_sync_all();  // nobody leaves while the peer may still multicast into / signal this CTA
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// ====================================================================================================================
-// cta_group::2 ("pair") kernel: two CTAs of a 2x1x1 cluster (one TPC) run ONE 256 x 256 UMMA tile.  Each CTA stages only
-// its own 128 rows of A and HALF of the B tile (128 of the 256 N-rows), so per k-block a CTA writes 32 KiB into shared
-// memory instead of 48 KiB and the MMA reads 8 KiB instead of 12 KiB per k16 step: shared-memory traffic drops from
-// ~192 B/clk (above the 128 B/clk port, the limiter of the single-CTA kernel at ~60-67 % tensor-pipe) to ~128 B/clk, and
-// the ring deepens from 4 to 6 stages.  Only the leader CTA (cluster rank 0) issues tcgen05.mma; both CTAs' TMA loads
-// complete on the LEADER's "full" barrier; tcgen05.commit is multicast to both CTAs ("empty" + accumulator-ready
-// barriers); both CTAs' epilogue warps arrive on the leader's "accumulator drained" barrier.
-// ====================================================================================================================
-constexpr int P_STAGES = 6;
-constexpr uint32_t P_A_BYTES = BLOCK_M * BLOCK_K * 2;         // 16 KiB: this CTA's 128 rows of A
-constexpr uint32_t P_B_BYTES = (BLOCK_N / 2) * BLOCK_K * 2;   // 16 KiB: this CTA's half of the B tile
-constexpr uint32_t P_STAGE_BYTES = P_A_BYTES + P_B_BYTES;     // 32 KiB
-constexpr int EPI_PITCH = 36;                                  // floats per staged row: 16-byte aligned, conflict-free
-constexpr uint32_t P_EPI_BYTES = 4 * 32 * EPI_PITCH * 4;       // one 32 x 32 fp32 transposition tile per epilogue warp
-constexpr uint32_t P_SMEM_BYTES = P_STAGES * P_STAGE_BYTES + 1024 + 256 + P_EPI_BYTES;
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;                // shared::cluster address of the same offset in CTA rank 0
-
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* map, uint64_t* leader_bar, void* smem_dst, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(map), "r"(smem_u32(leader_bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-
-// kExact: compile-time copy of EpiParams::exact_main — the plain instantiation keeps the double-buffered accumulator
-// bookkeeping and the single-accumulator epilogue as constants (the bf16 mode's inner loops carry none of the
-// exact mode's selects).
-template <bool kExact>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_bf16_tc_pair_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                         const __grid_constant__ CUtensorMap tmap_bh, EpiParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t* smem_a = smem;                                // P_STAGES x 16 KiB
-  uint8_t* smem_b = smem + P_STAGES * P_A_BYTES;         // P_STAGES x 16 KiB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + P_STAGES * P_STAGE_BYTES);
-  uint64_t* full_bar = bars;                             // [P_STAGES]   (used in the leader only)
-  uint64_t* empty_bar = bars + P_STAGES;                 // [P_STAGES]   (one per CTA, signalled by the leader's commits)
-  uint64_t* tmem_full = bars + 2 * P_STAGES;             // [ACC_STAGES] (one per CTA)
-  uint64_t* tmem_empty = bars + 2 * P_STAGES + ACC_STAGES;  // [ACC_STAGES] (leader only; 8 arrivals = 4 warps x 2 CTAs)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * P_STAGES + 2 * ACC_STAGES);
-  float* epi_tiles = reinterpret_cast<float*>(smem + P_STAGES * P_STAGE_BYTES + 256);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();
-  const bool leader = crank == 0;
-  const int m_tiles = (p.M + 2 * BLOCK_M - 1) / (2 * BLOCK_M);  // 256-row tiles
-  const int n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int num_units = m_tiles * n_tiles;
+  const int wg = warp >> 2;
+  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
+  const int tm = (int)(blockIdx.x % (unsigned)m_tiles), tn = (int)(blockIdx.x / (unsigned)m_tiles);
   const int k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
   const int kchunk = (p.kchunk > 0 && p.kchunk < k_blocks) ? p.kchunk : max(k_blocks, 1);
   const int n_chunks = max(1, (k_blocks + kchunk - 1) / kchunk);
-  constexpr int n_acc = kExact ? 1 : ACC_STAGES;   // exact: both TMEM buffers belong to one accumulator stage
-  const int unit0 = blockIdx.x / 2, unit_stride = gridDim.x / 2;
-  // Wave-quantisation fix: the units of the last, partially filled round are split into two 256 x 128 HALF units when
-  // that fills the idle CTA pairs (e.g. 4096^2: 256 units on 74 pairs = 3 full rounds + 34 -> 68 half units, 3.5 rounds
-  // instead of 4).  The work list is: full units [0, full_units), then half units; all roles walk the same sequence.
-  // (Measured: a half unit costs ~0.9 of a full one because it re-reads the whole A tile for half the flops, so the gain
-  // is 1-7 %; splitting K instead, with the two partial tiles combined through global memory, measured slower.)
-  const int rem = num_units % unit_stride;
-  const bool split_tail = p.split_tail && rem > 0 && 2 * rem <= unit_stride && num_units > unit_stride;
-  const int full_units = split_tail ? num_units - rem : num_units;
-  const int seq_len = full_units + (split_tail ? 2 * rem : 0);
 
-  // work item `seq` -> tile row, first column, half-unit flag
-#define PTK_DECODE_UNIT(seq, tm, ncol0, half)                                     \
-  int tm, ncol0;                                                                  \
-  bool half;                                                                      \
-  {                                                                               \
-    half = (seq) >= full_units;                                                   \
-    const int h_ = ((seq) - full_units) & 1;                                      \
-    const int u_ = half ? full_units + ((seq) - full_units) / 2 : (seq);          \
-    tm = u_ % m_tiles;                                                            \
-    ncol0 = (u_ / m_tiles) * BLOCK_N + (half ? h_ * (BLOCK_N / 2) : 0);           \
-  }
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
-    prefetch_tmap(&tmap_bh);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < P_STAGES; ++s) {
+    for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < ACC_STAGES; ++a) {
-      mbar_init(&tmem_full[a], 1);
-      mbar_init(&tmem_empty[a], 8);
+      mbar_init(&empty_bar[s], 8);
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc_2sm(tmem_ptr, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
-    // ===== TMA producer (both CTAs): own A rows + own half of B, completion counted on the LEADER's full barrier =====
-    if (lane == 0) {
+  if (wg == 0) {
+    // ===== TMA producer: one thread streams k-block x piece-product stages in the consumers' order =====
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int sq = unit0; sq < seq_len; sq += unit_stride) {
-        PTK_DECODE_UNIT(sq, tm, ncol0, half)
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          for (int t = 6 - p.terms; t < 6; ++t) {   // one ring stage per piece product (a single pass when terms == 1)
-            const int arow = kPieceA[t] * p.a_rows, brow = kPieceB[t] * p.b_rows;
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            if (leader) mbar_expect_tx(&full_bar[stage], half ? 2 * (P_A_BYTES + P_B_BYTES / 2) : 2 * P_STAGE_BYTES);
-            tma_load_2d_2sm(&tmap_a, &full_bar[stage], smem_a + stage * P_A_BYTES, kb * BLOCK_K,
-                            arow + tm * 2 * BLOCK_M + (int)crank * BLOCK_M);
-            if (half)  // this CTA's 64 of the 128 B rows of a half unit
-              tma_load_2d_2sm(&tmap_bh, &full_bar[stage], smem_b + stage * P_B_BYTES, kb * BLOCK_K,
-                              brow + ncol0 + (int)crank * (BLOCK_N / 4));
-            else
-              tma_load_2d_2sm(&tmap_b, &full_bar[stage], smem_b + stage * P_B_BYTES, kb * BLOCK_K,
-                              brow + ncol0 + (int)crank * (BLOCK_N / 2));
-            if (++stage == P_STAGES) { stage = 0; phase ^= 1; }
-          }
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        for (int t = 6 - p.terms; t < 6; ++t) {   // one ring stage per piece product (a single pass when terms == 1)
+          const int arow = kPieceA[t] * p.a_rows, brow = kPieceB[t] * p.b_rows;
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
+          tma_load_2d(&tmap_a, &full_bar[stage], smem_a + stage * A_STAGE_BYTES, kb * BLOCK_K, arow + tm * BLOCK_M);
+          tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * B_STAGE_BYTES, kb * BLOCK_K, brow + tn * BLOCK_N);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer: ONE thread of the leader CTA drives both SMs' tensor cores =====
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc_full = make_idesc(2 * BLOCK_M, BLOCK_N);
-      constexpr uint32_t idesc_half = make_idesc(2 * BLOCK_M, BLOCK_N / 2);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      constexpr bool exact = kExact;
-      const int terms_m1 = p.terms - 1;
-      for (int sq = unit0; sq < seq_len; sq += unit_stride) {
-        const uint32_t idesc = (sq >= full_units) ? idesc_half : idesc_full;
-        for (int ch = 0; ch < n_chunks; ++ch) {   // one TMEM accumulator per accumulation chunk (EpiParams::kchunk)
-          mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + (uint32_t)acc * BLOCK_N;
-          const uint32_t d_corr = tmem_base + (uint32_t)BLOCK_N;   // exact_main: the correction products' accumulator
-          const int kb_n = min(kchunk, k_blocks - ch * kchunk);
-          const int n_stages = kb_n * p.terms;  // piece products of one k-block accumulate into the same tile
-          int term = 0;                         // position inside the k-block's term sequence (no division in this loop:
-          for (int it = 0; it < n_stages; ++it) {   // one thread feeds both SMs' tensor cores, its latency is the pipe's)
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            const uint32_t a_addr = smem_u32(smem_a + stage * P_A_BYTES);
-            const uint32_t b_addr = smem_u32(smem_b + stage * P_B_BYTES);
-            // term order within a k-block: the correction products first, A1 x B1 last (kPieceA / kPieceB)
-            const bool to_corr = exact && term != terms_m1;
-            const uint32_t d_use = to_corr ? d_corr : d_tmem;
-            const bool first = exact ? (to_corr ? it == 0 : it == terms_m1) : it == 0;
-            term = (term == terms_m1) ? 0 : term + 1;
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-              umma_f16_2sm(d_use, make_smem_desc(a_addr + k * UMMA_K * 2), make_smem_desc(b_addr + k * UMMA_K * 2), idesc,
-                           (!first || k > 0) ? 1u : 0u);
-            }
-            umma_commit_2sm_mc(&empty_bar[stage], (uint16_t)0x3);  // the stage is free again in BOTH CTAs
-            if (++stage == P_STAGES) { stage = 0; phase ^= 1; }
-          }
-          umma_commit_2sm_mc(&tmem_full[acc], (uint16_t)0x3);      // accumulator complete in both CTAs' TMEM
-          if (++acc == n_acc) { acc = 0; acc_phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue (both CTAs): this CTA's 128 rows of the 256-row tile =====
-    const int q = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int sq = unit0; sq < seq_len; sq += unit_stride) {
-      PTK_DECODE_UNIT(sq, tm, ncol0, half)
-      const int ncols = half ? BLOCK_N / 2 : BLOCK_N;
-      const long long row = (long long)tm * 2 * BLOCK_M + (long long)crank * BLOCK_M + q * 32 + lane;
-      const bool row_ok = row < p.M;
-      float* crow = p.C + row * p.sc0;
-      const bool vec_ok = p.sc1 == 1 && (p.sc0 & 3) == 0 && (((uintptr_t)p.C) & 15) == 0 &&
-                          (p.Cbf == nullptr || ((p.ldcbf & 3) == 0 && (((uintptr_t)p.Cbf) & 7) == 0));
-#pragma unroll 1
-      for (int ch = 0; ch < n_chunks; ++ch) {
-        // chunk 0 combines with the caller's C (beta), later chunks add onto the partial sum this thread stored before;
-        // bias / activation / the bf16 copy belong to the completed sum
-        const float beta = ch == 0 ? p.beta : 1.0f;
-        const bool last = ch == n_chunks - 1;
-        const float* bias = last ? p.bias : nullptr;
-        const int act = last ? p.act : 0;
-        __nv_bfloat16* cbf = last ? p.Cbf : nullptr;
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c0 = 0; c0 < ncols; c0 += 32) {
-          uint32_t r[32];
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BLOCK_N + c0);
-          tmem_ld_32x32b_x32(taddr, r);
-          if constexpr (kExact) {
-            uint32_t r2[32];
-            tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(BLOCK_N + c0), r2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(r2[j]));
-          } else {
-            tmem_ld_wait();
-          }
-          const long long col0 = (long long)ncol0 + c0;
-          // Row-contiguous fast path (warp-uniform): tcgen05.ld hands every lane one ROW of the 32 x 32 block; going through
-          // a shared-memory tile turns that into 128 contiguous bytes of one row per quarter warp, so every global
-          // load / store instruction of the warp covers 4 full 128-byte lines (the read-modify-write of the accumulation
-          // chunks and the bf16 / three-piece operand copies move whole sectors instead of 16-byte shards of 32 lines).
-          if (vec_ok && col0 + 32 <= p.N && beta == 0.0f && (cbf == nullptr || p.out_pieces == 1)) {
-            // Store-only epilogue (nothing to read back, at most a bf16 copy): each lane keeps its ROW of the block and
-            // writes it as eight independent 16-byte groups — no shared-memory round trip, no warp barriers, eight-way
-            // instruction-level parallelism through the tanh chains.  The strided 16-byte stores are fire-and-forget; with
-            // a bias + tanh + bf16-copy epilogue this path keeps up with the next tile's MMAs where the row-contiguous one
-            // below (which pays off as soon as old values must be LOADED) does not (cfg3: 0.43 vs 0.47 ms).
-            if (row_ok) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                float4 v;
-                float* vv = reinterpret_cast<float*>(&v);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  float x = p.alpha * __uint_as_float(r[j + e]);
-                  if (bias) x += bias[col0 + j + e];
-                  if (act == 1) x = tanhf(x);
-                  vv[e] = x;
-                }
-                *reinterpret_cast<float4*>(crow + col0 + j) = v;
-                if (cbf) {
-                  __nv_bfloat162 lo = __floats2bfloat162_rn(vv[0], vv[1]), hi = __floats2bfloat162_rn(vv[2], vv[3]);
-                  uint2 pk;
-                  pk.x = *reinterpret_cast<uint32_t*>(&lo);
-                  pk.y = *reinterpret_cast<uint32_t*>(&hi);
-                  *reinterpret_cast<uint2*>(cbf + row * p.ldcbf + col0 + j) = pk;
-                }
-              }
-            }
-          } else if (vec_ok && col0 + 32 <= p.N) {
-            float* tile = epi_tiles + (warp - 4) * (32 * EPI_PITCH);
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              *reinterpret_cast<float4*>(tile + lane * EPI_PITCH + j) =
-                  make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-            __syncwarp();
-            const int sub = lane >> 3, cq = (lane & 7) * 4;
-            const long long colv = col0 + cq;
-            float bb[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-            if (bias) {
-#pragma unroll
-              for (int e = 0; e < 4; ++e) bb[e] = bias[colv + e];
-            }
-            const long long row_base = (long long)tm * 2 * BLOCK_M + (long long)crank * BLOCK_M + q * 32;
-            // the old values of all 8 row groups are requested before any of them is used (and before any store of this
-            // block, which the compiler could not prove disjoint): one memory round trip per 32 x 32 block, not eight
-            float4 old[8];
-            if (beta != 0.0f) {
-#pragma unroll
-              for (int g = 0; g < 8; ++g) {
-                const long long grow = row_base + 4 * g + sub;
-                old[g] = grow < p.M ? __ldcg(reinterpret_cast<const float4*>(p.C + grow * p.sc0 + colv)) : make_float4(0.f, 0.f, 0.f, 0.f);
-              }
-            }
-#pragma unroll
-            for (int g = 0; g < 8; ++g) {
-              const int rr = 4 * g;
-              const long long grow = row_base + rr + sub;
-              if (grow < p.M) {
-                float4 v = *reinterpret_cast<const float4*>(tile + (rr + sub) * EPI_PITCH + cq);
-                float* dst = p.C + grow * p.sc0 + colv;
-                float vv[4] = {p.alpha * v.x, p.alpha * v.y, p.alpha * v.z, p.alpha * v.w};
-                if (beta != 0.0f) {
-                  vv[0] += beta * old[g].x; vv[1] += beta * old[g].y; vv[2] += beta * old[g].z; vv[3] += beta * old[g].w;
-                }
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  vv[e] += bb[e];
-                  if (act == 1) vv[e] = tanhf(vv[e]);
-                }
-                *reinterpret_cast<float4*>(dst) = make_float4(vv[0], vv[1], vv[2], vv[3]);
-                if (cbf) {
-                  for (int pc = 0; pc < p.out_pieces; ++pc) {   // piece pc = bf16 of what the earlier pieces left over
-                    if (pc == 0 && p.out_exp != PTK_NO_EXP) {     // aligned leading piece (exact in bf16)
-#pragma unroll
-                      for (int e = 0; e < 4; ++e) {
-                        const float lead = rintf(vv[e] * p.out_scale) * p.out_inv;
-                        vv[e] -= lead;
-                        reinterpret_cast<float*>(&v)[e] = lead;
-                      }
-                      __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
-                      uint2 pk;
-                      pk.x = *reinterpret_cast<uint32_t*>(&lo);
-                      pk.y = *reinterpret_cast<uint32_t*>(&hi);
-                      *reinterpret_cast<uint2*>(cbf + ((long long)pc * p.cbf_rows + grow) * p.ldcbf + colv) = pk;
-                      continue;
-                    }
-                    __nv_bfloat162 lo = __floats2bfloat162_rn(vv[0], vv[1]), hi = __floats2bfloat162_rn(vv[2], vv[3]);
-                    uint2 pk;
-                    pk.x = *reinterpret_cast<uint32_t*>(&lo);
-                    pk.y = *reinterpret_cast<uint32_t*>(&hi);
-                    *reinterpret_cast<uint2*>(cbf + ((long long)pc * p.cbf_rows + grow) * p.ldcbf + colv) = pk;
-                    vv[0] -= __bfloat162float(lo.x); vv[1] -= __bfloat162float(lo.y);
-                    vv[2] -= __bfloat162float(hi.x); vv[3] -= __bfloat162float(hi.y);
-                  }
-                }
-              }
-            }
-            __syncwarp();
-          } else if (row_ok && col0 < p.N) {
-            {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const long long col = col0 + j;
-                if (col < p.N) {
-                  float* dst = crow + col * p.sc1;
-                  float x = p.alpha * __uint_as_float(r[j]);
-                  if (beta != 0.0f) x += beta * (*dst);
-                  if (bias) x += bias[col];
-                  if (act == 1) x = tanhf(x);
-                  *dst = x;
-                  if (cbf) {
-                    for (int pc = 0; pc < p.out_pieces; ++pc) {
-                      const __nv_bfloat16 b = (pc == 0 && p.out_exp != PTK_NO_EXP)
-                                                  ? __float2bfloat16_rn(rintf(x * p.out_scale) * p.out_inv)
-                                                  : __float2bfloat16_rn(x);
-                      cbf[((long long)pc * p.cbf_rows + row) * p.ldcbf + col] = b;
-                      x -= __bfloat162float(b);
-                    }
-                  }
-                }
-              }
-            }
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_leader(&tmem_empty[acc]);  // 8 arrivals (4 warps x 2 CTAs) free the accumulator
-        if (++acc == n_acc) { acc = 0; acc_phase ^= 1; }
-      }
-    }
+    return;
   }
-#undef PTK_DECODE_UNIT
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, TMEM_COLS);
+
+  // ===== consumers: warpgroup 1 -> rows [0, 64) of the tile, warpgroup 2 -> rows [64, 128) =====
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1;
+  float acc[64];
+  float cor[kExact ? 64 : 1];
+  int stage = 0;
+  uint32_t phase = 0;
+  const int terms_m1 = p.terms - 1;
+  const long long row0 = (long long)tm * BLOCK_M + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+  const long long col0 = (long long)tn * BLOCK_N + (lane & 3) * 2;
+#pragma unroll 1
+  for (int ch = 0; ch < n_chunks; ++ch) {
+    const int kb_n = min(kchunk, k_blocks - ch * kchunk);
+    const int n_stages = kb_n * p.terms;   // piece products of one k-block accumulate into the same tile
+    if (n_stages == 0) {                   // K == 0: the product is zero
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] = 0.0f;
+    }
+    int term = 0;                          // position inside the k-block's term sequence
+    int prev = -1;                         // stage whose wgmmas may still be reading shared memory
+#pragma unroll 1
+    for (int it = 0; it < n_stages; ++it) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_addr = smem_u32(smem_a + stage * A_STAGE_BYTES + cw * (64 * BLOCK_K * 2));
+      const uint32_t b_addr = smem_u32(smem_b + stage * B_STAGE_BYTES);
+      // term order within a k-block: the correction products first, A1 x B1 last (kPieceA / kPieceB)
+      const bool to_corr = kExact && term != terms_m1;
+      const bool first = kExact ? (to_corr ? it == 0 : it == terms_m1) : it == 0;
+      term = (term == terms_m1) ? 0 : term + 1;
+      wg_fence();
+      fence_regs(acc);
+      if constexpr (kExact) fence_regs(cor);
+      if constexpr (kExact) {
+        if (to_corr) {
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / WG_K; ++k)
+            wgmma_m64n128k16(cor, make_smem_desc(a_addr + k * WG_K * 2), make_smem_desc(b_addr + k * WG_K * 2),
+                             (!first || k > 0) ? 1u : 0u);
+        } else {
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / WG_K; ++k)
+            wgmma_m64n128k16(acc, make_smem_desc(a_addr + k * WG_K * 2), make_smem_desc(b_addr + k * WG_K * 2),
+                             (!first || k > 0) ? 1u : 0u);
+        }
+      } else {
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / WG_K; ++k)
+          wgmma_m64n128k16(acc, make_smem_desc(a_addr + k * WG_K * 2), make_smem_desc(b_addr + k * WG_K * 2),
+                           (!first || k > 0) ? 1u : 0u);
+      }
+      wg_commit();
+      wg_wait<1>();   // the previous stage's wgmmas are complete: its shared memory may be refilled
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wg_wait<0>();
+    fence_regs(acc);
+    if constexpr (kExact) fence_regs(cor);
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    if constexpr (kExact) {
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] += cor[j];
+    }
+    // chunk 0 combines with the caller's C (beta), later chunks add onto the partial sum this thread stored before;
+    // bias / activation / the bf16 copy belong to the completed sum
+    const float beta = ch == 0 ? p.beta : 1.0f;
+    const bool last = ch == n_chunks - 1;
+    const float* bias = last ? p.bias : nullptr;
+    const int act = last ? p.act : 0;
+    __nv_bfloat16* cbf = last ? p.Cbf : nullptr;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        epi_pair(p, row0 + 8 * h, col0 + 8 * j, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], beta, bias, act, cbf);
+    }
   }
 }
 
@@ -986,6 +590,22 @@ ptk_status make_tmap(CUtensorMap* m, const void* base, uint64_t rows, uint64_t c
 
 inline long long round_up(long long x, long long m) { return (x + m - 1) / m * m; }
 
+// One CTA per 128 x 128 tile of C; A and B^T are bf16 K-major matrices behind the two tensor maps.
+ptk_status launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const EpiParams& p, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    PTK_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+    PTK_CUDA(cudaFuncSetAttribute(gemm_bf16_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+    attr_set = true;
+  }
+  const long long tiles = (long long)((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + BLOCK_N - 1) / BLOCK_N);
+  if (tiles > 2147483647LL) return ptk::fail(PTK_ERR_ARG, "gemm_tc: too many output tiles");
+  if (p.exact_main) gemm_bf16_wgmma_kernel<true><<<(unsigned)tiles, NUM_THREADS, SMEM_BYTES, st>>>(ta, tb, p);
+  else gemm_bf16_wgmma_kernel<false><<<(unsigned)tiles, NUM_THREADS, SMEM_BYTES, st>>>(ta, tb, p);
+  PTK_LAUNCH_CHECK("gemm_bf16_wgmma");
+  return PTK_OK;
+}
+
 }  // namespace
 
 namespace ptk {
@@ -1021,8 +641,6 @@ static int exact_main_default() {
   return g;
 }
 
-static int g_cluster = -1;  // -1: read PTK_GEMM_CLUSTER once (default 2)
-
 // A_f32 (any strides) OR A_bf16 (row-major, pitch lda_bf16 elements, multiple of 8, 16-byte aligned base) must be given.
 ptk_status gemm_tc_ex(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t sa0, int64_t sa1,
                       const void* A_bf16, int64_t lda_bf16, const float* B, int64_t sb0, int64_t sb1, float beta, float* C,
@@ -1032,10 +650,6 @@ ptk_status gemm_tc_ex(int64_t M, int64_t N, int64_t K, float alpha, const float*
   if (M > 2147483647LL || N > 2147483647LL || K > 2147483647LL) return fail(PTK_ERR_ARG, "gemm_tc: dims exceed int32");
   if (workspace == nullptr || workspace_bytes < gemm_tc_workspace(M, N, K))
     return fail(PTK_ERR_ARG, "gemm_tc: workspace too small (see ptk_gemm_workspace_bytes)");
-  if (g_cluster < 0) {
-    const char* e = getenv("PTK_GEMM_MODE");  // 1 = single CTA, 2 = CTA pair sharing B by TMA multicast, 3 = cta_group::2 UMMA
-    g_cluster = (e && e[0] >= '1' && e[0] <= '3') ? (e[0] - '0') : 3;
-  }
   const long long Kp = round_up(K, 8);
   uintptr_t w = ((uintptr_t)workspace + 255) & ~(uintptr_t)255;
   __nv_bfloat16* Abf = reinterpret_cast<__nv_bfloat16*>(w);
@@ -1055,57 +669,17 @@ ptk_status gemm_tc_ex(int64_t M, int64_t N, int64_t K, float alpha, const float*
     convert_bf16_kernel<<<gb, 256, 0, st>>>(B, sb1, sb0, Bbf, Kp, N, K);
     PTK_LAUNCH_CHECK("convert_bf16");
   }
-  const int cluster = g_cluster;
-  CUtensorMap ta, tb, tbh;
+  CUtensorMap ta, tb;
   ptk_status s;
   if ((s = make_tmap(&ta, Abf, (uint64_t)M, (uint64_t)K, (uint64_t)lda, BLOCK_M)) != PTK_OK) return s;
-  if ((s = make_tmap(&tbh, Bbf, (uint64_t)N, (uint64_t)K, (uint64_t)Kp, BLOCK_N / 4)) != PTK_OK) return s;
-  if ((s = make_tmap(&tb, Bbf, (uint64_t)N, (uint64_t)K, (uint64_t)Kp, cluster >= 2 ? BLOCK_N / 2 : BLOCK_N)) != PTK_OK) return s;
+  if ((s = make_tmap(&tb, Bbf, (uint64_t)N, (uint64_t)K, (uint64_t)Kp, BLOCK_N)) != PTK_OK) return s;
   EpiParams p;
   p.alpha = alpha; p.beta = beta; p.C = C; p.sc0 = sc0; p.sc1 = sc1; p.bias = bias; p.act = act;
   p.M = (int)M; p.N = (int)N; p.K = (int)K;
   p.Cbf = reinterpret_cast<__nv_bfloat16*>(C_bf16);
   p.ldcbf = ldc_bf16;
-  static int g_split = -1;
-  if (g_split < 0) {
-    const char* e = getenv("PTK_GEMM_SPLIT");
-    g_split = (e && e[0] == '0') ? 0 : 1;
-  }
-  p.split_tail = g_split;
   p.terms = 1; p.a_rows = 0; p.b_rows = 0; p.kchunk = 0; p.out_pieces = 1; p.cbf_rows = 0; p.exact_main = 0; p.out_exp = PTK_NO_EXP; p.out_scale = 1.0f; p.out_inv = 1.0f;
-  static bool attr_set = false;
-  if (!attr_set) {
-    PTK_CUDA(cudaFuncSetAttribute(gemm_bf16_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    PTK_CUDA(cudaFuncSetAttribute(gemm_bf16_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    PTK_CUDA(cudaFuncSetAttribute(gemm_bf16_tc_pair_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P_SMEM_BYTES));
-    PTK_CUDA(cudaFuncSetAttribute(gemm_bf16_tc_pair_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P_SMEM_BYTES));
-    attr_set = true;
-  }
-  const int m_tiles = (int)((M + BLOCK_M - 1) / BLOCK_M), n_tiles = (int)((N + BLOCK_N - 1) / BLOCK_N);
-  const int sms = std::max(2, ptk::sm_count());
-  if (cluster >= 2) {
-    const int units = ((m_tiles + 1) / 2) * n_tiles;
-    const int grid = 2 * std::max(1, std::min(units, sms / 2));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = cluster == 3 ? P_SMEM_BYTES : SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (cluster == 3) PTK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_tc_pair_kernel<false>, ta, tb, tbh, p));
-    else PTK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_tc_kernel<2>, ta, tb, p));
-  } else {
-    const int grid = std::max(1, std::min(m_tiles * n_tiles, sms));
-    gemm_bf16_tc_kernel<1><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(ta, tb, p);
-  }
-  PTK_LAUNCH_CHECK("gemm_bf16_tc");
-  return PTK_OK;
+  return launch_gemm(ta, tb, p, st);
 }
 
 // accumulation chunk of the fp32-accurate modes: 8 k-blocks (K = 512) keeps the tensor core's truncation bias near 1e-6 of
@@ -1149,7 +723,7 @@ ptk_status stage_operand(const float* src, int64_t sr, int64_t sc, int64_t R, in
   return PTK_OK;
 }
 
-// The cta_group::2 kernel over operands that are ALREADY staged (see stage_operand): A_stage = pieces of A [M,K] (K-major,
+// The tensor-core kernel over operands that are ALREADY staged (see stage_operand): A_stage = pieces of A [M,K] (K-major,
 // pitch lda, piece pitch a_rows rows), B_stage = pieces of B^T [N,K]; terms 1 (plain bf16) | 3 | 6.  C_stage (optional)
 // receives `out_pieces` (1 | 3) staged pieces of the RESULT [M,N] (pitch ldc_stage, piece pitch c_rows) — the A operand
 // of the next product of a chain / recurrence, so that only the very first operand is ever staged by a separate pass.
@@ -1165,12 +739,11 @@ ptk_status gemm_tc_staged(int64_t M, int64_t N, int64_t K, float alpha, const vo
   if (C_stage != nullptr && (out_pieces != 1 && out_pieces != 3)) return fail(PTK_ERR_ARG, "gemm_tc_staged: out_pieces must be 1 or 3");
   if (C_stage != nullptr && (ldc_stage % 8 || ((uintptr_t)C_stage & 15))) return fail(PTK_ERR_ARG, "gemm_tc_staged: misaligned C_stage");
   const int pa = terms == 1 ? 1 : 3;
-  CUtensorMap ta, tb, tbh;
+  CUtensorMap ta, tb;
   ptk_status s;
   const uint64_t a_total = (uint64_t)((pa - 1) * a_rows + M), b_total = (uint64_t)((pa - 1) * b_rows + N);
   if ((s = make_tmap(&ta, A_stage, a_total, (uint64_t)K, (uint64_t)lda, BLOCK_M)) != PTK_OK) return s;
-  if ((s = make_tmap(&tbh, B_stage, b_total, (uint64_t)K, (uint64_t)ldb, BLOCK_N / 4)) != PTK_OK) return s;
-  if ((s = make_tmap(&tb, B_stage, b_total, (uint64_t)K, (uint64_t)ldb, BLOCK_N / 2)) != PTK_OK) return s;
+  if ((s = make_tmap(&tb, B_stage, b_total, (uint64_t)K, (uint64_t)ldb, BLOCK_N)) != PTK_OK) return s;
   EpiParams p;
   p.alpha = alpha; p.beta = beta; p.C = C; p.sc0 = sc0; p.sc1 = sc1; p.bias = bias; p.act = act;
   p.M = (int)M; p.N = (int)N; p.K = (int)K;
@@ -1179,7 +752,6 @@ ptk_status gemm_tc_staged(int64_t M, int64_t N, int64_t K, float alpha, const vo
   p.out_pieces = C_stage ? out_pieces : 1;
   p.cbf_rows = c_rows;
   p.exact_main = 0; p.out_exp = PTK_NO_EXP; p.out_scale = 1.0f; p.out_inv = 1.0f;
-  p.split_tail = 1;
   p.terms = terms; p.a_rows = terms == 1 ? 0 : (int)a_rows; p.b_rows = terms == 1 ? 0 : (int)b_rows;
   p.exact_main = (terms != 1 && exact_main) ? 1 : 0;
   p.out_exp = (C_stage && out_pieces == 3) ? out_exp : PTK_NO_EXP;
@@ -1189,36 +761,11 @@ ptk_status gemm_tc_staged(int64_t M, int64_t N, int64_t K, float alpha, const vo
     p.out_inv = ldexpf(1.0f, -p.out_exp);
   }
   p.kchunk = terms == 1 ? 0 : split_kchunk(K, p.exact_main);
-  static bool attr_set = false;
-  if (!attr_set) {
-    PTK_CUDA(cudaFuncSetAttribute(gemm_bf16_tc_pair_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P_SMEM_BYTES));
-    PTK_CUDA(cudaFuncSetAttribute(gemm_bf16_tc_pair_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P_SMEM_BYTES));
-    attr_set = true;
-  }
-  const int m_tiles = (int)((M + BLOCK_M - 1) / BLOCK_M), n_tiles = (int)((N + BLOCK_N - 1) / BLOCK_N);
-  const int sms = std::max(2, ptk::sm_count());
-  const int units = ((m_tiles + 1) / 2) * n_tiles;
-  const int grid = 2 * std::max(1, std::min(units, sms / 2));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = P_SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (p.exact_main) PTK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_tc_pair_kernel<true>, ta, tb, tbh, p));
-  else PTK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_tc_pair_kernel<false>, ta, tb, tbh, p));
-  PTK_LAUNCH_CHECK("gemm_tc_staged");
-  return PTK_OK;
+  return launch_gemm(ta, tb, p, st);
 }
 
 // fp32-accurate product on the tensor cores: both operands split into three bf16 pieces, `terms` (3 or 6) piece products
-// per k-block accumulated in fp32 TMEM by the cta_group::2 kernel (see EpiParams::terms).
+// per k-block accumulated in fp32 registers by the wgmma kernel (see EpiParams::terms).
 ptk_status gemm_tc_split(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t sa0, int64_t sa1, const float* B,
                          int64_t sb0, int64_t sb1, float beta, float* C, int64_t sc0, int64_t sc1, const float* bias, int act,
                          int terms, void* workspace, size_t workspace_bytes, cudaStream_t st) {
@@ -1238,49 +785,22 @@ ptk_status gemm_tc_split(int64_t M, int64_t N, int64_t K, float alpha, const flo
     if ((ss = stage_operand(A, sa0, sa1, M, K, 3, Abf, Kp, Mp, exact, sexp, st)) != PTK_OK) return ss;
     if ((ss = stage_operand(B, sb1, sb0, N, K, 3, Bbf, Kp, Np, exact, sexp + M, st)) != PTK_OK) return ss;  // B[K,N] -> Bt[N,K]
   }
-  CUtensorMap ta, tb, tbh;
+  CUtensorMap ta, tb;
   ptk_status s;
   // rows past M (N) inside a piece hold whatever the workspace held: they only reach output rows (columns) the epilogue
   // masks, never a stored element; columns past K are zero-filled by TMA (the map's extent is K)
   if ((s = make_tmap(&ta, Abf, (uint64_t)(3 * Mp), (uint64_t)K, (uint64_t)Kp, BLOCK_M)) != PTK_OK) return s;
-  if ((s = make_tmap(&tbh, Bbf, (uint64_t)(3 * Np), (uint64_t)K, (uint64_t)Kp, BLOCK_N / 4)) != PTK_OK) return s;
-  if ((s = make_tmap(&tb, Bbf, (uint64_t)(3 * Np), (uint64_t)K, (uint64_t)Kp, BLOCK_N / 2)) != PTK_OK) return s;
+  if ((s = make_tmap(&tb, Bbf, (uint64_t)(3 * Np), (uint64_t)K, (uint64_t)Kp, BLOCK_N)) != PTK_OK) return s;
   EpiParams p;
   p.alpha = alpha; p.beta = beta; p.C = C; p.sc0 = sc0; p.sc1 = sc1; p.bias = bias; p.act = act;
   p.M = (int)M; p.N = (int)N; p.K = (int)K;
   p.Cbf = nullptr;
   p.ldcbf = 0;
   p.out_pieces = 1; p.cbf_rows = 0; p.exact_main = 0; p.out_exp = PTK_NO_EXP; p.out_scale = 1.0f; p.out_inv = 1.0f;
-  p.split_tail = 1;
   p.terms = terms; p.a_rows = (int)Mp; p.b_rows = (int)Np;
   p.exact_main = exact;
   p.kchunk = split_kchunk(K, exact);
-  static bool attr_set = false;
-  if (!attr_set) {
-    PTK_CUDA(cudaFuncSetAttribute(gemm_bf16_tc_pair_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P_SMEM_BYTES));
-    PTK_CUDA(cudaFuncSetAttribute(gemm_bf16_tc_pair_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)P_SMEM_BYTES));
-    attr_set = true;
-  }
-  const int m_tiles = (int)((M + BLOCK_M - 1) / BLOCK_M), n_tiles = (int)((N + BLOCK_N - 1) / BLOCK_N);
-  const int sms = std::max(2, ptk::sm_count());
-  const int units = ((m_tiles + 1) / 2) * n_tiles;
-  const int grid = 2 * std::max(1, std::min(units, sms / 2));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = P_SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (p.exact_main) PTK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_tc_pair_kernel<true>, ta, tb, tbh, p));
-  else PTK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_tc_pair_kernel<false>, ta, tb, tbh, p));
-  PTK_LAUNCH_CHECK("gemm_bf16x3_tc");
-  return PTK_OK;
+  return launch_gemm(ta, tb, p, st);
 }
 
 ptk_status gemm_tc(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t sa0, int64_t sa1,

@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(256) put_rows_kernel(T* __restrict__ dst, cons
 inline unsigned grid_for(int64_t total, int threads = 256) {
   int64_t blocks = (total + threads - 1) / threads;
   int64_t cap = (int64_t)ptk::sm_count() * 16;
-  if (cap <= 0) cap = 148 * 16;
+  if (cap <= 0) cap = 132 * 16;  // H100 SXM
   return (unsigned)std::max<int64_t>(1, std::min(blocks, cap));
 }
 

@@ -114,9 +114,9 @@ ptk_status ptk_init(int device) {
   PTK_CUDA(cudaFree(0));
   cudaDeviceProp prop;
   PTK_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     return fail(PTK_ERR_UNSUPPORTED, std::string("ptk_init: device '") + prop.name +
-                                         "' is not sm_100 class; libptk is built for sm_100a only");
+                                         "' is not sm_90 class; libptk is built for sm_90a (H100) only");
   }
   g_sms = prop.multiProcessorCount;
   ptk_status s;
@@ -183,7 +183,7 @@ ptk_status ptk_jit_compile(const char* src, const char* const* opts, int n_opts,
   nvrtcResult r = g_rtc.CreateProgram(&prog, src, "ptk_jit.cu", 0, nullptr, nullptr);
   if (r != NVRTC_SUCCESS) return fail(PTK_ERR_NVRTC, std::string("nvrtcCreateProgram: ") + g_rtc.GetErrorString(r));
   std::vector<const char*> o;
-  o.push_back("--gpu-architecture=sm_100a");
+  o.push_back("--gpu-architecture=sm_90a");
   o.push_back("--std=c++17");
   o.push_back("-lineinfo");
   o.push_back("-default-device");

@@ -1,4 +1,4 @@
-"""`pytensor.link.cuda` — the B200 CUDA backend package (aliased into the `pytensor.link` namespace on registration).
+"""`pytensor.link.cuda` — the H100 CUDA backend package (aliased into the `pytensor.link` namespace on registration).
 
 Registration uses the reference's own hooks: `register_linker` / `register_mode` (pytensor/compile/mode.py:59,624)
 and the inner-graph `singledispatch`es every linker must register with (`rewrite_scan_inner_graph`,

@@ -1,4 +1,4 @@
-"""`CUDALinker`: the B200 execution backend behind PyTensor's Linker plugin surface.
+"""`CUDALinker`: the H100 execution backend behind PyTensor's Linker plugin surface.
 
 Boundary (reference file:line):
   * `Linker` / `LocalLinker` ABCs — pytensor/link/basic.py:138,228 (`make_thunk` :235-246 returns
@@ -176,12 +176,12 @@ class CudaVM:
 
 
 class CUDALinker(LocalLinker):
-    """Linker whose VM keeps every intermediate in HBM and runs hand-written sm_100a kernels through libptk.
+    """Linker whose VM keeps every intermediate in HBM and runs hand-written sm_90a kernels through libptk.
 
     Parameters
     ----------
-    gemm_precision : "fp32" (native FMA, <=1e-5 vs the C linker) or "bf16" (tcgen05 tensor cores: operands rounded to
-        bf16, fp32 accumulation in TMEM; parity vs the C linker at the half-precision tolerance, see DESIGN.md).
+    gemm_precision : "fp32" (native FMA, <=1e-5 vs the C linker) or "bf16" (wgmma tensor cores: operands rounded to
+        bf16, fp32 accumulation; parity vs the C linker at the half-precision tolerance, see DESIGN.md).
     device_outputs : return torch.cuda tensors instead of NumPy arrays (no device->host copy, no sync).
     """
 

@@ -2,7 +2,7 @@
 
 This is the backend's analogue of `Op.make_thunk` (pytensor/graph/op.py:610-659) / `COp.make_c_thunk`
 (pytensor/link/c/op.py:38-106): it is called once per node at link time, and raises `NotImplementedError` for any
-op without an sm_100a implementation — compile-time, never a CPU fallback (SURVEY.md §7 step 1).
+op without an sm_90a implementation — compile-time, never a CPU fallback (SURVEY.md §7 step 1).
 """
 
 from __future__ import annotations
@@ -80,7 +80,7 @@ def scalar_program(scalar_op, in_dtypes, out_dtypes) -> ScalarProgram:
             return [ref_of(o)[0] for o in fg.outputs]
         name = type(op).__name__
         if name not in OPS:
-            raise UnsupportedOp(f"scalar op {name} ({op}) has no sm_100a device expression")
+            raise UnsupportedOp(f"scalar op {name} ({op}) has no sm_90a device expression")
         if len(out_types) != 1:
             raise UnsupportedOp(f"multi-output scalar op {name}")
         prog.insts.append(ScalarInst(name, list(arg_refs), list(arg_dtypes), out_types[0]))
@@ -347,6 +347,6 @@ def lower_node(node, opts):
         return lower_scan(node, opts)
 
     raise UnsupportedOp(
-        f"CUDALinker: op {op} ({type(op).__module__}.{type(op).__name__}) has no sm_100a implementation; "
+        f"CUDALinker: op {op} ({type(op).__module__}.{type(op).__name__}) has no sm_90a implementation; "
         "the CUDA backend never falls back to the CPU"
     )

@@ -1,5 +1,5 @@
 """Build-time kernel cache warm-up: trace the BASELINE workloads in trace-only mode (runtime/lib.py TRACE_ONLY) so that
-every NVRTC kernel they launch is compiled for sm_100a into `pytensor_b200/_kcache/` on the CPU-only build box."""
+every NVRTC kernel they launch is compiled for sm_90a into the in-tree cache `pytensor_b200/_kcache/` (needs no GPU)."""
 
 from __future__ import annotations
 
@@ -31,8 +31,9 @@ def precompile_workloads(verbose=True):
     from pytensor_b200 import workloads as W
     from pytensor_b200.runtime import jit
 
-    old = pytensor.config.floatX
+    old, old_dir = pytensor.config.floatX, jit.CACHE_DIR
     pytensor.config.floatX = "float32"
+    jit.CACHE_DIR = jit.BUILD_CACHE_DIR
     try:
         jobs = [("cfg2", W.cfg2_fused_elemwise(4096), "CUDA"), ("cfg2-smoke", W.cfg2_fused_elemwise(512), "CUDA"),
                 ("cfg1", W.cfg1_readme(1024), "CUDA")]
@@ -43,4 +44,4 @@ def precompile_workloads(verbose=True):
             if verbose:
                 print(f"[precompile] {name}: {n} launches traced; cache stats {jit.stats}")
     finally:
-        pytensor.config.floatX = old
+        pytensor.config.floatX, jit.CACHE_DIR = old, old_dir

@@ -24,7 +24,7 @@ def require_cuda() -> None:
     if _lib.TRACE_ONLY:
         return
     if not torch.cuda.is_available():
-        raise _lib.PtkError("the CUDA backend needs a B200 (torch.cuda.is_available() is False); there is no CPU fallback")
+        raise _lib.PtkError("the CUDA backend needs an H100 (torch.cuda.is_available() is False); there is no CPU fallback")
 
 
 _device = None

@@ -1,9 +1,13 @@
 """NVRTC-backed kernel cache.
 
 The reference compiles one C++ module per Apply node with g++ and caches it on disk keyed by op/type signature
-(pytensor/link/c/cmodule.py:612 ModuleCache, :1181-1260 module_from_key).  The B200 analogue: one sm_100a cubin per
-generated kernel source, cached in memory per process and on disk (in-tree `_kcache/`, so that cubins built by
-`__graft_entry__.build()` travel to the GPU box) keyed by the SHA-256 of (source, options).
+(pytensor/link/c/cmodule.py:612 ModuleCache, :1181-1260 module_from_key).  The H100 analogue: one sm_90a cubin per
+generated kernel source, cached in memory per process and on disk keyed by the SHA-256 of (architecture, source,
+options).  Two disk caches: the in-tree `_kcache/` that `__graft_entry__.build()` fills (read-only afterwards, so that a
+run from a read-only tree still starts with cache hits) and a per-user directory under the system temporary directory
+(PTK_KCACHE overrides it) that receives everything compiled at run time.  A cached cubin is trusted by its file name, so
+the shared-temp default is used only when it is a real directory owned by this user and closed to everyone else (it is
+created with mode 0700); otherwise kernels compiled at run time are cached in memory only.
 """
 
 from __future__ import annotations
@@ -11,13 +15,16 @@ from __future__ import annotations
 import ctypes
 import hashlib
 import os
+import stat
+import tempfile
 import threading
 
 from . import lib as _lib
 
-CACHE_DIR = os.environ.get(
-    "PTK_KCACHE", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "_kcache")
-)
+ARCH = "sm_90a"  # the architecture ptk_jit_compile targets (csrc/ptk_runtime.cu)
+BUILD_CACHE_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "_kcache")
+DEFAULT_CACHE_DIR = os.path.join(tempfile.gettempdir(), f"ptk_kcache_{os.getuid()}")
+CACHE_DIR = os.environ.get("PTK_KCACHE") or DEFAULT_CACHE_DIR
 
 _lock = threading.Lock()
 _cubins: dict[str, bytes] = {}
@@ -28,9 +35,23 @@ stats = {"compiled": 0, "disk_hits": 0, "mem_hits": 0, "launches": 0}
 
 def _key(src: str, opts: tuple[str, ...]) -> str:
     h = hashlib.sha256()
-    h.update(("ptk-jit-v1\0" + "\0".join(opts) + "\0").encode())
+    h.update(("ptk-jit-v2\0" + ARCH + "\0" + "\0".join(opts) + "\0").encode())
     h.update(src.encode())
     return h.hexdigest()[:32]
+
+
+def _usable_cache_dir() -> str | None:
+    """CACHE_DIR, created (mode 0700) if missing; None when it is the shared-temp default but not a directory that only
+    this user can write (someone else could have planted cubins there)."""
+    d = CACHE_DIR
+    try:
+        os.makedirs(d, mode=0o700, exist_ok=True)
+        st = os.lstat(d)
+    except OSError:
+        return None
+    if d == DEFAULT_CACHE_DIR and (not stat.S_ISDIR(st.st_mode) or st.st_uid != os.getuid() or st.st_mode & 0o077):
+        return None
+    return d
 
 
 def compile_cubin(src: str, opts: tuple[str, ...] = ()) -> tuple[str, bytes]:
@@ -40,14 +61,18 @@ def compile_cubin(src: str, opts: tuple[str, ...] = ()) -> tuple[str, bytes]:
         if key in _cubins:
             stats["mem_hits"] += 1
             return key, _cubins[key]
-    path = os.path.join(CACHE_DIR, key + ".cubin")
-    if os.path.exists(path):
-        with open(path, "rb") as f:
-            data = f.read()
-        with _lock:
-            _cubins[key] = data
-            stats["disk_hits"] += 1
-        return key, data
+    cache_dir = _usable_cache_dir()
+    candidates = [os.path.join(BUILD_CACHE_DIR, key + ".cubin")]
+    if cache_dir is not None:
+        candidates.insert(0, os.path.join(cache_dir, key + ".cubin"))
+    for p in dict.fromkeys(candidates):
+        if os.path.exists(p):
+            with open(p, "rb") as f:
+                data = f.read()
+            with _lock:
+                _cubins[key] = data
+                stats["disk_hits"] += 1
+            return key, data
     L = _lib.load_library()
     cubin = ctypes.c_void_p()
     size = ctypes.c_size_t()
@@ -63,16 +88,17 @@ def compile_cubin(src: str, opts: tuple[str, ...] = ()) -> tuple[str, bytes]:
         raise _lib.PtkError(f"NVRTC failed: {_lib.last_error()}\n{log_txt}\n--- source ---\n{numbered}")
     data = ctypes.string_at(cubin.value, size.value)
     L.ptk_free(cubin)
-    try:
-        os.makedirs(CACHE_DIR, exist_ok=True)
-        tmp = path + f".tmp{os.getpid()}"
-        with open(tmp, "wb") as f:
-            f.write(data)
-        os.replace(tmp, path)
-        with open(os.path.join(CACHE_DIR, key + ".cu"), "w") as f:
-            f.write(src)
-    except OSError:
-        pass
+    if cache_dir is not None:
+        try:
+            path = os.path.join(cache_dir, key + ".cubin")
+            tmp = path + f".tmp{os.getpid()}"
+            with open(tmp, "wb") as f:
+                f.write(data)
+            os.replace(tmp, path)
+            with open(os.path.join(cache_dir, key + ".cu"), "w") as f:
+                f.write(src)
+        except OSError:
+            pass
     with _lock:
         _cubins[key] = data
         stats["compiled"] += 1

@@ -1,7 +1,7 @@
 """ctypes binding of libptk.so (the C-ABI declared in include/ptk.h).
 
 There is exactly one way to compute in this package: through these entry points.  If the shared library is missing
-or no B200 is present, every compute call raises — there is no CPU or PyTorch fallback anywhere in the product path.
+or no H100 is present, every compute call raises — there is no CPU or PyTorch fallback anywhere in the product path.
 """
 
 from __future__ import annotations
@@ -126,7 +126,7 @@ TRACE_ONLY = os.environ.get("PTK_TRACE_ONLY") == "1"
 class _TraceLib:
     def __getattr__(self, name):
         if name == "ptk_sm_count":
-            return lambda: 148
+            return lambda: 132  # H100 SXM
         if name == "ptk_gemm_workspace_bytes":
             return lambda M, N, K, p: 2 * (M * K + N * K) + 1024
         if name == "ptk_put_rows_workspace_bytes":

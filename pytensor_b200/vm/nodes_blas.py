@@ -1,6 +1,6 @@
 """BLAS-family nodes (reference: pytensor/tensor/blas/gemm.py:76 Gemm, :248 Dot22, :298 Dot22Scalar,
 gemv.py:16 Gemv, ger.py:8 Ger, and the generic Dot of pytensor/tensor/math.py).  All arithmetic runs in
-ptk_gemm / ptk_gemv / ptk_ger; `precision` selects the bf16 tcgen05 tensor-core path for fp32 matrices."""
+ptk_gemm / ptk_gemv / ptk_ger; `precision` selects the bf16 wgmma tensor-core path for fp32 matrices."""
 
 from __future__ import annotations
 
@@ -13,9 +13,9 @@ from .nodes_basic import _broadcast_view
 from .nodes_elemwise import Node
 from .values import Val
 
-# Linker-level knob: 0 = fp32-accurate (<= 1e-5 vs BLAS); 1 = bf16 operands / fp32 TMEM accumulation
+# Linker-level knob: 0 = fp32-accurate (<= 1e-5 vs BLAS); 1 = bf16 operands / fp32 accumulation
 TC_MIN_DIM = 256
-# How precision 0 multiplies large fp32 matrices: "tc6" / "tc3" = tcgen05 with every operand split into three bf16 pieces
+# How precision 0 multiplies large fp32 matrices: "tc6" / "tc3" = wgmma with every operand split into three bf16 pieces
 # and 6 / 3 piece products per k-block (include/ptk.h ptk_gemm_tc_split; 6 terms is more accurate than sgemm itself,
 # 3 terms ~4e-6 of the output scale), "simt" = the fp32 FMA kernel.  fp64 and small / skinny products always take FMA.
 import os as _os

@@ -1,6 +1,6 @@
-"""Micro-benchmark of the bf16 tcgen05 GEMM through the C-ABI (ptk_gemm_tc_ex) with A already in bf16 (the chained-layer
-case): the conversion of B and the GEMM kernel are timed together and, with ncu, separately.
-usage: python scripts/gemm_bench.py [M N K]...   (env PTK_GEMM_MODE / PTK_GEMM_SPLIT select the kernel variant)"""
+"""Micro-benchmark of the bf16 tensor-core (wgmma) GEMM through the C-ABI (ptk_gemm_tc_ex) with A already in bf16 (the chained-layer
+case): the conversion of B and the GEMM kernel are timed together.
+usage: python scripts/gemm_bench.py [M N K]..."""
 import os
 import sys
 
@@ -38,5 +38,5 @@ for M, N, K in shapes:
     ms = e0.elapsed_time(e1) / n
     ref = Abf.float() @ B.bfloat16().float()
     err = ((C - ref).abs().max() / ref.abs().max()).item()
-    print(f"M={M} N={N} K={K} split={os.environ.get('PTK_GEMM_SPLIT', '1')} {ms*1e3:.1f} us (incl. B convert) "
+    print(f"M={M} N={N} K={K} {ms*1e3:.1f} us (incl. B convert) "
           f"{2*M*N*K/ms/1e9:.0f} TF/s  rel.err {err:.2e}", flush=True)

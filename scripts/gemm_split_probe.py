@@ -1,4 +1,4 @@
-"""fp32-accurate tcgen05 GEMM (ptk_gemm_tc_split) through the C-ABI: error against an fp64 product and time per call.
+"""fp32-accurate tensor-core GEMM (ptk_gemm_tc_split) through the C-ABI: error against an fp64 product and time per call.
 The accumulation chunk (EpiParams::kchunk) is read once per process from PTK_GEMM_KCHUNK: run once per setting.
 usage: PTK_GEMM_KCHUNK=8 python scripts/gemm_split_probe.py [terms]"""
 import os

@@ -1,10 +1,10 @@
 """Static instruction count of the cfg2 map+row-reduce kernel (K3): generates the kernel exactly as `mode="CUDA"` would
 (trace-only mode + NVRTC, no GPU needed), disassembles the cubin and reports the SASS size of its loops — the main loop
-processes 8 elements per thread and trip.  The kernel is instruction-issue bound (profiles/r2_prof_k3_final_ncu_summary.csv:
-issue-active 73 %), so instructions per element are the quantity that matters.
+processes 8 elements per thread and trip.  Where the kernel is instruction-issue bound, instructions per element are the
+quantity that matters.
 
     python scripts/k3_sass_count.py                      # shipped configuration
-    PTK_K3_ADDR=idx PTK_SCALAR_SIMPLIFY=0 python scripts/k3_sass_count.py   # the round's measured kernel (39.2 us)
+    PTK_K3_ADDR=idx PTK_SCALAR_SIMPLIFY=0 python scripts/k3_sass_count.py   # index addressing, no scalar simplification
 """
 import collections
 import os

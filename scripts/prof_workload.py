@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Run a BASELINE workload a few times eagerly (for `ncu` launch lists / full captures).  usage: prof_workload.py cfg3|cfg4|cfg5|metric [steps]"""
+"""Run a BASELINE workload a few times eagerly (a target for a profiler).  usage: prof_workload.py cfg3|cfg4|cfg5|metric [steps]"""
 import os
 import sys
 

@@ -1,7 +1,6 @@
 """NumPy model of the fp32-accurate tensor-core GEMM (DESIGN.md §4 K4x), kept beside the kernel as the statement of WHY it
-works.  The device accumulates bf16 x bf16 products into an fp32 accumulator that TRUNCATES (measured on the B200: a
-systematic shrink of about 1e-7 per accumulation step, profiles/r2_gemm_split_kchunk_probe.txt).  The model reproduces that
-accumulator and shows, on the same operands:
+works.  The tensor core accumulates bf16 x bf16 products into an fp32 accumulator that may TRUNCATE (a systematic shrink
+of about 1e-7 per accumulation step).  The model reproduces such an accumulator and shows, on the same operands:
 
   * the plain three-piece split (x1 = bf16(x), ...) inherits the shrink: the result is biased towards zero by ~K * 2^-24;
   * with error-free leading pieces (x1 = rint(x * 2^s) * 2^-s, |rint| <= 2^7, s per row of A / column of B) every A1*B1

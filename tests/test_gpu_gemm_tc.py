@@ -1,4 +1,4 @@
-"""The bf16 tcgen05/TMEM GEMM path (K4/K5) against the reference C linker's fp32 sgemm.
+"""The bf16 tensor-core (wgmma) GEMM path (K4/K5) against the reference C linker's fp32 sgemm.
 
 Tolerance: operands are rounded to bf16 (8-bit mantissa, rel 2^-9 per operand), products accumulate in fp32, so a
 K-term dot product of O(1) values carries an absolute error ~ sqrt(K) * 2^-9 * |a||b|.  This is the reference's own
@@ -21,10 +21,8 @@ def _check(got, ref, K):
     assert err < 4e-3, f"bf16 tensor-core GEMM deviates {err:.2e} of the output scale (K={K})"
 
 
-# the last three shapes have more 256x256 units than CTA pairs (148 SMs -> 74 pairs) with a remainder that is split into
-# 256x128 half units (wave-quantisation path of gemm_bf16_tc_pair_kernel): 80 units (6 -> 12 halves), ragged 80 units,
-# and 12 x 13 = 156 units (8 -> 16 halves, two full rounds before the tail); the last two have >= 8 k-blocks, which the
-# split-K variant of the tail (PTK_GEMM_SPLIT=2) requires
+# the last shapes have more 128x128 output tiles than the H100 has SMs (132), ragged M / N / K edges included, and the
+# last two have >= 8 k-blocks
 @pytest.mark.parametrize("M,N,K", [(256, 256, 256), (512, 768, 320), (1000, 520, 264), (384, 256, 1024),
                                    (2560, 2048, 256), (2500, 2000, 264), (3072, 3328, 320),
                                    (2500, 2000, 520), (2560, 2048, 1032)])

@@ -160,6 +160,9 @@ def test_row_batched_gather_and_deterministic_scatter_add(gpu, dtype):
     out = pt.inc_subtensor(pt.zeros_like(theta)[:, g], r)
     f, got = compare_cuda_and_cvm([theta, r, g], [out], [tv, rv, gv], rtol=1e-6 if dtype == "float32" else 1e-13,
                                   atol=1e-5 if dtype == "float32" else 1e-12)
+    # the scatter-add runs inside a row-fused region (codegen/rowfuse.py), so the bit-exact check below covers its
+    # lane-ordered accumulation
+    assert any(type(s.impl).__name__ == "RowRegionNode" for s in f.vm.executor.program.steps)
     ref = np.zeros_like(tv)
     np.add.at(ref, (slice(None), gv), rv)
     np.testing.assert_array_equal(got[0], ref)  # deterministic: same accumulation order as np.add.at

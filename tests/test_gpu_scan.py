@@ -51,7 +51,7 @@ def _contractive(args, gain=0.6):
 @pytest.mark.parametrize("full_trace", [False, True])
 @pytest.mark.parametrize("rows,cols,steps", [(300, 256, 9), (512, 384, 25)])
 def test_matmul_recurrence_on_tensor_cores_chained_operands(gpu, rows, cols, steps, full_trace):
-    """dims >= 256: the fp32-accurate tcgen05 path — W staged once, every step's epilogue writes the three-piece staged
+    """dims >= 256: the fp32-accurate tensor-core path — W staged once, every step's epilogue writes the three-piece staged
     operand of the next step (nodes_scan_matmul.py); final state (2-slot circular buffer) and full trace, vs the C linker."""
     pytensor.config.floatX = "float32"
     from pytensor_b200 import workloads as W

@@ -1,5 +1,5 @@
 """CPU suite: every BASELINE.json config lowers under mode="CUDA" and its launch logic runs in trace-only mode
-(NVRTC compiles each generated kernel for sm_100a; no device, no results)."""
+(NVRTC compiles each generated kernel for sm_90a; no device, no results)."""
 
 import numpy as np
 import pytest
@@ -101,7 +101,7 @@ def test_cfg5_and_metric_graph_lower():
 
 def test_unsupported_ops_fail_at_compile_time_not_at_run_time():
     x = pt.dmatrix("x")
-    with pytest.raises(NotImplementedError, match="no sm_100a implementation"):
+    with pytest.raises(NotImplementedError, match="no sm_90a implementation"):
         pytensor.function([x], pt.linalg.inv(x), mode="CUDA")
     c = pt.zmatrix("c")
     with pytest.raises(NotImplementedError):

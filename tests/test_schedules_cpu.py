@@ -1,52 +1,11 @@
-"""CPU checks of two scheduling rules that the CUDA kernels implement in index arithmetic (Python mirrors of the device
-code; the kernels themselves are covered by the -m gpu parity tests):
+"""CPU check of a scheduling rule that a CUDA kernel implements in index arithmetic (a Python mirror of the device
+code; the kernel itself is covered by the -m gpu parity tests):
 
-  * the persistent pair-GEMM's work list with the tail split into half units (gemm_bf16_tc_pair_kernel,
-    csrc/ptk_gemm_tc.cu: PTK_DECODE_UNIT) must cover every output tile exactly once;
   * the fused Scan kernel's run-based walk of a circular trace buffer (codegen/scan.py) must write step i to slot
     (L + i) % store, like the reference's circular buffers (pytensor/scan/scan_perform.pyx:544-570).
 """
 
-import itertools
-
 import numpy as np
-
-
-def _pair_gemm_cover(M, N, n_pairs_hw, split=True, BM=128, BN=256):
-    m_tiles = (M + 2 * BM - 1) // (2 * BM)
-    n_tiles = (N + BN - 1) // BN
-    num_units = m_tiles * n_tiles
-    stride = max(1, min(num_units, n_pairs_hw))          # gridDim.x / 2
-    rem = num_units % stride
-    split_tail = split and rem > 0 and 2 * rem <= stride and num_units > stride
-    full_units = num_units - rem if split_tail else num_units
-    seq_len = full_units + (2 * rem if split_tail else 0)
-    cover = np.zeros((m_tiles, n_tiles * BN), dtype=np.int32)
-    per_pair = np.zeros(stride)
-    for pair in range(stride):
-        for sq in range(pair, seq_len, stride):
-            half = sq >= full_units
-            h = (sq - full_units) & 1
-            u = full_units + (sq - full_units) // 2 if half else sq
-            tm, col0 = u % m_tiles, (u // m_tiles) * BN + (h * (BN // 2) if half else 0)
-            ncols = BN // 2 if half else BN
-            cover[tm, col0:col0 + ncols] += 1
-            per_pair[pair] += 0.5 if half else 1.0
-    return cover, per_pair, split_tail
-
-
-def test_pair_gemm_work_list_covers_every_tile_once():
-    for M, N, pairs in itertools.product([256, 1000, 2500, 2560, 3072, 4096, 8192], [256, 520, 2000, 2048, 3328, 4096],
-                                         [74, 66, 4, 1]):
-        for split in (False, True):
-            cover, per_pair, split_tail = _pair_gemm_cover(M, N, pairs, split)
-            assert (cover == 1).all(), (M, N, pairs, split)
-            if split_tail:  # the split must shorten the critical path (units of the busiest pair)
-                _, base, _ = _pair_gemm_cover(M, N, pairs, False)
-                assert per_pair.max() == base.max() - 0.5, (M, N, pairs)
-    # the shape the MLP benchmark runs: 256 units on 74 pairs -> 3 full rounds + 68 half units
-    _, per_pair, split_tail = _pair_gemm_cover(4096, 4096, 74)
-    assert split_tail and per_pair.max() == 3.5
 
 
 def _scan_slots(T, store, L):
