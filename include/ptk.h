@@ -206,6 +206,13 @@ ptk_status   ptk_gemm_tc_split(int64_t M, int64_t N, int64_t K, double alpha, co
  *     out_pieces (1 | 3) staged pieces of the result [M,N] (pitch ldc_stage, piece pitch c_rows); out_exp != PTK_STAGE_NO_EXP
  *     aligns the leading output piece to that fixed exponent (results known to lie in [-1, 1], e.g. tanh),
  *     which makes the pieces a valid `aligned` A operand of a following exact_main product.
+ *     ±inf operands: a three-piece ptk_stage_operand at the default pitches leaves one word per row behind the pieces
+ *     (at ptk_stage_bytes(rows, cols, 3) - 256 - 4 * rows from the 256-aligned dst): the row's largest magnitude, whose
+ *     bits are 0x7f800000 (+inf) for a row with ±inf.
+ *     a_flags / b_flags (nullable) are those words of A and B^T; the outputs of a flagged row / column are then summed from
+ *     the pieces in fp32, giving sgemm's ±inf / NaN instead of the NaN of inf * 0 piece products.  c_flags (nullable,
+ *     zeroed by the caller, 3-piece C_stage only) receives the same flags for the rows of C_stage.  An epilogue-written
+ *     operand carries flags only through c_flags.
  *   ptk_gemm_exact_main_default: 1 unless PTK_GEMM_EXACT=0 — what ptk_gemm_tc_split uses. */
 #define PTK_STAGE_NO_EXP (-100000)
 size_t       ptk_stage_bytes(int64_t rows, int64_t cols, int pieces);
@@ -214,7 +221,8 @@ ptk_status   ptk_stage_operand(const void* src_f32, int64_t sr, int64_t sc, int6
 ptk_status   ptk_gemm_tc_staged(int64_t M, int64_t N, int64_t K, double alpha, const void* A_stage, int64_t lda, int64_t a_rows,
                       const void* B_stage, int64_t ldb, int64_t b_rows, int terms, double beta, void* C, int64_t sc0,
                       int64_t sc1, const void* bias, int act, void* C_stage, int64_t ldc_stage, int64_t c_rows,
-                      int out_pieces, int exact_main, int out_exp, void* stream);
+                      int out_pieces, int exact_main, int out_exp, const void* a_flags, const void* b_flags,
+                      void* c_flags, void* stream);
 int          ptk_gemm_exact_main_default(void);
 /* Width b of the aligned leading piece for a contraction of length K (|leading integer| <= 2^b; 7 today for every K);
  * out_exp of a chained tanh epilogue feeding a product of contraction length K' is ptk_gemm_lead_bits(K') - 1. */

@@ -161,11 +161,43 @@ struct EpiParams {
   // in [-1, 1]) so that it can feed an exact-main product; PTK_NO_EXP: ordinary bf16 split
   int out_exp;
   float out_scale, out_inv;   // 2^out_exp and 2^-out_exp (exact powers of two: the alignment is two multiplies and a rint)
+  // ±inf operands (fp32-accurate modes).  An infinite x is staged as (x, 0, 0), so the piece products that pair it with a
+  // zero piece of the other operand are inf * 0 = NaN where sgemm has ±inf.  fa / fb flag the rows of A / columns of B
+  // that hold ±inf (kInfBits, the row maximum row_absmax_kernel leaves; null = no flags): a consumer thread owning such an
+  // output skips its epilogue, and nonfinite_fixup_kernel recomputes that thread's outputs from the staged pieces As / Bs
+  // (pitch lda / ldb, piece pitch a_rows / b_rows).  fc (nullable, zeroed by the caller) receives the same flags for the
+  // rows of a three-piece Cbf.
+  const unsigned int* fa;
+  const unsigned int* fb;
+  unsigned int* fc;
+  const __nv_bfloat16* As;
+  const __nv_bfloat16* Bs;
+  long long lda, ldb;
 };
 #define PTK_NO_EXP (-100000)
+constexpr unsigned int kInfBits = 0x7f800000u;
 // piece indices of the term sequence; a run of `terms` entries ending at index 5 is used
 __device__ __constant__ int kPieceA[6] = {2, 1, 0, 1, 0, 0};
 __device__ __constant__ int kPieceB[6] = {0, 1, 2, 0, 1, 0};
+
+// sum over k of A[row, k] * B[k, col], each operand rebuilt exactly from its three staged pieces (p0 + p1 + p2), products
+// summed in fp64 and rounded once: the outputs nonfinite_fixup_kernel recomputes.  ±inf / NaN come out as sgemm has them.
+__device__ float nonfinite_dot(const __nv_bfloat16* As, long long lda, long long a_rows, const __nv_bfloat16* Bs, long long ldb,
+                               long long b_rows, int K, long long row, long long col) {
+  const __nv_bfloat16* a = As + row * lda;
+  const __nv_bfloat16* b = Bs + col * ldb;
+  double s = 0.0;
+  for (int k = 0; k < K; ++k) {
+    const double x = (double)__bfloat162float(a[k]) + (double)__bfloat162float(a[a_rows * lda + k]) +
+                     (double)__bfloat162float(a[2 * a_rows * lda + k]);
+    const double y = (double)__bfloat162float(b[k]) + (double)__bfloat162float(b[b_rows * ldb + k]) +
+                     (double)__bfloat162float(b[2 * b_rows * ldb + k]);
+    s = fma(x, y, s);
+  }
+  return (float)s;
+}
+
+__device__ __forceinline__ bool inf_flagged(const unsigned int* f, long long i) { return f != nullptr && f[i] == kInfBits; }
 
 // One output element pair (row, col), (row, col + 1) of a finished chunk: alpha * acc (+ beta * C) (+ bias) (tanh), the
 // bf16 / three-piece copy.  The vector and the scalar branch compute the same values.
@@ -201,13 +233,15 @@ __device__ __forceinline__ void epi_pair(const EpiParams& p, long long row, long
     if (two) dst[p.sc1] = x[1];
   }
   if (cbf) {
+    const float inf = __int_as_float(kInfBits), bfmax = __int_as_float(0x7f7f0000);   // (bfmax: the largest bf16)
+    if (p.fc != nullptr && (fabsf(x[0]) == inf || (two && fabsf(x[1]) == inf))) p.fc[row] = kInfBits;
     for (int pc = 0; pc < p.out_pieces; ++pc) {   // piece pc = bf16 of what the earlier pieces left over
       __nv_bfloat16 b[2];
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         b[e] = (pc == 0 && p.out_exp != PTK_NO_EXP) ? __float2bfloat16_rn(rintf(x[e] * p.out_scale) * p.out_inv)
-                                                    : __float2bfloat16_rn(x[e]);
-        x[e] -= __bfloat162float(b[e]);
+                                                    : __float2bfloat16_rn(fabsf(x[e]) < inf ? fminf(fmaxf(x[e], -bfmax), bfmax) : x[e]);
+        x[e] = fabsf(x[e]) < inf ? x[e] - __bfloat162float(b[e]) : 0.0f;   // ±inf / NaN ride in the leading piece alone
       }
       __nv_bfloat16* d = cbf + ((long long)pc * p.cbf_rows + row) * p.ldcbf + col;
       if (two && ((((uintptr_t)d) & 3) == 0)) {
@@ -221,6 +255,18 @@ __device__ __forceinline__ void epi_pair(const EpiParams& p, long long row, long
       }
     }
   }
+}
+
+// Does this consumer thread own an output whose row of A or column of B holds ±inf?  (two rows, 32 columns)
+__device__ __forceinline__ bool thread_flagged(const unsigned int* fa, const unsigned int* fb, int M, int N, long long row0,
+                                            long long col0) {
+  bool any = false;
+  for (int h = 0; h < 2; ++h) any |= row0 + 8 * h < M && inf_flagged(fa, row0 + 8 * h);
+  for (int j = 0; j < 32; ++j) {
+    const long long col = col0 + 8 * (j >> 1) + (j & 1);
+    any |= col < N && inf_flagged(fb, col);
+  }
+  return any;
 }
 
 // kExact: compile-time copy of EpiParams::exact_main — the plain instantiation carries no second accumulator.
@@ -284,6 +330,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   const int terms_m1 = p.terms - 1;
   const long long row0 = (long long)tm * BLOCK_M + cw * 64 + (warp & 3) * 16 + (lane >> 2);
   const long long col0 = (long long)tn * BLOCK_N + (lane & 3) * 2;
+  // a thread owning an output whose row of A / column of B holds ±inf leaves all its outputs to nonfinite_fixup_kernel
+  const bool flagged = (p.fa != nullptr || p.fb != nullptr) && thread_flagged(p.fa, p.fb, p.M, p.N, row0, col0);
 #pragma unroll 1
   for (int ch = 0; ch < n_chunks; ++ch) {
     const int kb_n = min(kchunk, k_blocks - ch * kchunk);
@@ -345,11 +393,37 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
     const float* bias = last ? p.bias : nullptr;
     const int act = last ? p.act : 0;
     __nv_bfloat16* cbf = last ? p.Cbf : nullptr;
+    if (flagged) continue;
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
 #pragma unroll
       for (int h = 0; h < 2; ++h)
         epi_pair(p, row0 + 8 * h, col0 + 8 * j, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], beta, bias, act, cbf);
+    }
+  }
+}
+
+// The outputs the GEMM kernel left alone (thread_flagged): one block per output tile, thread t standing for consumer thread
+// t of the GEMM (same fragment mapping), the GEMM's own epilogue over dot products from nonfinite_dot.  C still holds the
+// caller's values there, so beta, bias, tanh and the staged output pieces come out as for any other output.  A tile without
+// a flagged row or column costs one flag load per thread.
+__global__ void __launch_bounds__(256) nonfinite_fixup_kernel(const EpiParams p) {
+  const int m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
+  const int tm = (int)(blockIdx.x % (unsigned)m_tiles), tn = (int)(blockIdx.x / (unsigned)m_tiles);
+  const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+  const long long r = (long long)tm * BLOCK_M + (t & 127), c = (long long)tn * BLOCK_N + (t & 127);
+  const bool mine = t < 128 ? (r < p.M && inf_flagged(p.fa, r)) : (c < p.N && inf_flagged(p.fb, c));
+  if (!__syncthreads_or(mine)) return;
+  const long long row0 = (long long)tm * BLOCK_M + (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
+  const long long col0 = (long long)tn * BLOCK_N + (lane & 3) * 2;
+  if (!thread_flagged(p.fa, p.fb, p.M, p.N, row0, col0)) return;
+  for (int j = 0; j < 16; ++j) {
+    for (int h = 0; h < 2; ++h) {
+      const long long row = row0 + 8 * h, col = col0 + 8 * j;
+      if (row >= p.M || col >= p.N) continue;
+      const float v0 = nonfinite_dot(p.As, p.lda, p.a_rows, p.Bs, p.ldb, p.b_rows, p.K, row, col);
+      const float v1 = col + 1 < p.N ? nonfinite_dot(p.As, p.lda, p.a_rows, p.Bs, p.ldb, p.b_rows, p.K, row, col + 1) : 0.0f;
+      epi_pair(p, row, col, v0, v1, p.beta, p.bias, p.act, p.Cbf);
     }
   }
 }
@@ -402,6 +476,8 @@ __global__ void __launch_bounds__(256) convert_bf16_kernel(const float* __restri
 // ---- fp32 -> 3 x bf16 operand split: piece i of src[r*sr + c*sc] goes to dst[(i * piece_rows + r) * ld + c] ----------------
 // x1 = bf16(x), x2 = bf16(x - x1), x3 = bf16(x - x1 - x2): the residuals are exact in fp32, so x1 + x2 + x3 carries 24
 // mantissa bits of x.  Same 64 x 64 shared-memory tile as convert_bf16_kernel (coalesced reads along either source stride).
+// A non-finite x is staged as (x, 0, 0); a finite x beyond the largest bf16 (3.3895e38) gets that largest value as its
+// leading piece instead of inf, so that its remainder stays finite.
 __global__ void __launch_bounds__(256) split_bf16x3_kernel(const float* __restrict__ src, long long sr, long long sc,
                                                            __nv_bfloat16* __restrict__ dst, long long ld, long long R,
                                                            long long Cc, long long piece_rows) {
@@ -434,9 +510,11 @@ __global__ void __launch_bounds__(256) split_bf16x3_kernel(const float* __restri
     const long long r = r0 + ty + 8 * i, c = c0 + 2 * tx;
     if (r < R && c < Cc) {
       float lo = tile[ty + 8 * i][2 * tx], hi = (c + 1 < Cc) ? tile[ty + 8 * i][2 * tx + 1] : 0.0f;
+      const float inf = __int_as_float(0x7f800000), bfmax = __int_as_float(0x7f7f0000);
 #pragma unroll
       for (int pc = 0; pc < 3; ++pc) {
-        const __nv_bfloat16 bl = __float2bfloat16_rn(lo), bh = __float2bfloat16_rn(hi);
+        const __nv_bfloat16 bl = __float2bfloat16_rn(fabsf(lo) < inf ? fminf(fmaxf(lo, -bfmax), bfmax) : lo);
+        const __nv_bfloat16 bh = __float2bfloat16_rn(fabsf(hi) < inf ? fminf(fmaxf(hi, -bfmax), bfmax) : hi);
         __nv_bfloat16* d = dst + (pc * piece_rows + r) * ld + c;
         if (c + 1 < ld) {
           __nv_bfloat162 pk;
@@ -446,8 +524,8 @@ __global__ void __launch_bounds__(256) split_bf16x3_kernel(const float* __restri
         } else {
           *d = bl;
         }
-        lo -= __bfloat162float(bl);
-        hi -= __bfloat162float(bh);
+        lo = fabsf(lo) < inf ? lo - __bfloat162float(bl) : 0.0f;   // ±inf / NaN ride in the leading piece alone
+        hi = fabsf(hi) < inf ? hi - __bfloat162float(bh) : 0.0f;
       }
     }
   }
@@ -553,7 +631,10 @@ __global__ void __launch_bounds__(256) split_aligned_kernel(const float* __restr
       __nv_bfloat16 pc[3][2];
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        const float lead = rintf(v[e] * up) * dn;   // |rint| <= 128: exact in bf16; x - lead exact in fp32
+        const float q = rintf(v[e] * up);   // |q| <= 2^lead_bits: exact in bf16; x - lead exact in fp32
+        float lead = q * dn;
+        if (fabsf(lead) == __int_as_float(0x7f800000) && fabsf(v[e]) < __int_as_float(0x7f800000))
+          lead = (q - copysignf(1.0f, q)) * dn;   // the top binade: 2^lead_bits * 2^-sx = 2^128 overflows
         pc[0][e] = __float2bfloat16_rn(lead);
         float rem = v[e] - lead;
         if (!(fabsf(v[e]) < __int_as_float(0x7f800000))) rem = 0.0f;  // inf / NaN ride in the leading piece only
@@ -603,6 +684,10 @@ ptk_status launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const EpiPa
   if (p.exact_main) gemm_bf16_wgmma_kernel<true><<<(unsigned)tiles, NUM_THREADS, SMEM_BYTES, st>>>(ta, tb, p);
   else gemm_bf16_wgmma_kernel<false><<<(unsigned)tiles, NUM_THREADS, SMEM_BYTES, st>>>(ta, tb, p);
   PTK_LAUNCH_CHECK("gemm_bf16_wgmma");
+  if (p.fa != nullptr || p.fb != nullptr) {
+    nonfinite_fixup_kernel<<<(unsigned)tiles, 256, 0, st>>>(p);
+    PTK_LAUNCH_CHECK("nonfinite_fixup");
+  }
   return PTK_OK;
 }
 
@@ -679,6 +764,7 @@ ptk_status gemm_tc_ex(int64_t M, int64_t N, int64_t K, float alpha, const float*
   p.Cbf = reinterpret_cast<__nv_bfloat16*>(C_bf16);
   p.ldcbf = ldc_bf16;
   p.terms = 1; p.a_rows = 0; p.b_rows = 0; p.kchunk = 0; p.out_pieces = 1; p.cbf_rows = 0; p.exact_main = 0; p.out_exp = PTK_NO_EXP; p.out_scale = 1.0f; p.out_inv = 1.0f;
+  p.fa = p.fb = nullptr; p.fc = nullptr; p.As = p.Bs = nullptr; p.lda = p.ldb = 0;   // bf16 operands: inf * 0 = NaN is the model
   return launch_gemm(ta, tb, p, st);
 }
 
@@ -702,6 +788,8 @@ static int split_kchunk(int64_t K, int exact) {
 
 // Operand staging on its own (so that an operand that does not change between calls is staged ONCE): dst = `pieces` (1 | 3)
 // bf16 matrices [R, Cc] stacked with a pitch of piece_rows rows, row pitch ld elements, from fp32 src[r*sr + c*sc].
+// sexp (R words, required when aligned): the row maxima (row_absmax_kernel), which are +inf for a row holding ±inf — the
+// flags of EpiParams::fa / fb, kept for the plain split too.
 ptk_status stage_operand(const float* src, int64_t sr, int64_t sc, int64_t R, int64_t Cc, int pieces, void* dst, int64_t ld,
                          int64_t piece_rows, int aligned, int* sexp, cudaStream_t st) {
   if (pieces != 1 && pieces != 3) return fail(PTK_ERR_ARG, "stage_operand: pieces must be 1 or 3");
@@ -709,13 +797,15 @@ ptk_status stage_operand(const float* src, int64_t sr, int64_t sc, int64_t R, in
   if (ld % 8 != 0 || ld < Cc || ((uintptr_t)dst & 15) != 0) return fail(PTK_ERR_ARG, "stage_operand: pitch must be a multiple of 8 >= cols, base 16-byte aligned");
   if (R == 0 || Cc == 0) return PTK_OK;
   dim3 g((unsigned)((Cc + 63) / 64), (unsigned)((R + 63) / 64));
+  unsigned int* flags = reinterpret_cast<unsigned int*>(sexp);
+  if (pieces == 3 && flags != nullptr) {
+    PTK_CUDA(cudaMemsetAsync(flags, 0, (size_t)R * 4, st));
+    row_absmax_kernel<<<g, 256, 0, st>>>(src, sr, sc, R, Cc, flags);
+  }
   if (pieces == 1) {
     convert_bf16_kernel<<<g, 256, 0, st>>>(src, sr, sc, (__nv_bfloat16*)dst, ld, R, Cc);
   } else if (aligned) {
-    PTK_CUDA(cudaMemsetAsync(sexp, 0, (size_t)R * 4, st));
-    row_absmax_kernel<<<g, 256, 0, st>>>(src, sr, sc, R, Cc, reinterpret_cast<unsigned int*>(sexp));
-    split_aligned_kernel<<<g, 256, 0, st>>>(src, sr, sc, (__nv_bfloat16*)dst, ld, R, Cc, piece_rows,
-                                            reinterpret_cast<const unsigned int*>(sexp), lead_bits_for(Cc));
+    split_aligned_kernel<<<g, 256, 0, st>>>(src, sr, sc, (__nv_bfloat16*)dst, ld, R, Cc, piece_rows, flags, lead_bits_for(Cc));
   } else {
     split_bf16x3_kernel<<<g, 256, 0, st>>>(src, sr, sc, (__nv_bfloat16*)dst, ld, R, Cc, piece_rows);
   }
@@ -730,7 +820,8 @@ ptk_status stage_operand(const float* src, int64_t sr, int64_t sc, int64_t R, in
 ptk_status gemm_tc_staged(int64_t M, int64_t N, int64_t K, float alpha, const void* A_stage, int64_t lda, int64_t a_rows,
                           const void* B_stage, int64_t ldb, int64_t b_rows, int terms, float beta, float* C, int64_t sc0,
                           int64_t sc1, const float* bias, int act, void* C_stage, int64_t ldc_stage, int64_t c_rows,
-                          int out_pieces, int exact_main, int out_exp, cudaStream_t st) {
+                          int out_pieces, int exact_main, int out_exp, const unsigned int* a_flags,
+                          const unsigned int* b_flags, unsigned int* c_flags, cudaStream_t st) {
   if (M == 0 || N == 0) return PTK_OK;
   if (terms != 1 && terms != 3 && terms != 6) return fail(PTK_ERR_ARG, "gemm_tc_staged: terms must be 1, 3 or 6");
   if (M > 500000000LL || N > 500000000LL || K > 2147483647LL || K <= 0) return fail(PTK_ERR_ARG, "gemm_tc_staged: bad dims");
@@ -761,6 +852,11 @@ ptk_status gemm_tc_staged(int64_t M, int64_t N, int64_t K, float alpha, const vo
     p.out_inv = ldexpf(1.0f, -p.out_exp);
   }
   p.kchunk = terms == 1 ? 0 : split_kchunk(K, p.exact_main);
+  const bool three = terms != 1;   // (flags only mean something for three-piece operands / outputs)
+  p.fa = three ? a_flags : nullptr; p.fb = three ? b_flags : nullptr;
+  p.fc = (C_stage && out_pieces == 3) ? c_flags : nullptr;
+  p.As = reinterpret_cast<const __nv_bfloat16*>(A_stage); p.Bs = reinterpret_cast<const __nv_bfloat16*>(B_stage);
+  p.lda = lda; p.ldb = ldb;
   return launch_gemm(ta, tb, p, st);
 }
 
@@ -779,8 +875,8 @@ ptk_status gemm_tc_split(int64_t M, int64_t N, int64_t K, float alpha, const flo
   __nv_bfloat16* Abf = reinterpret_cast<__nv_bfloat16*>(w);
   __nv_bfloat16* Bbf = reinterpret_cast<__nv_bfloat16*>(w + round_up(3 * Mp * Kp * 2, 256));
   const int exact = terms == 6 ? exact_main_default() : 0;   // (3 terms need the 8-bit leading pieces of the plain split)
+  int* sexp = reinterpret_cast<int*>(w + round_up(3 * Mp * Kp * 2, 256) + round_up(3 * Np * Kp * 2, 256));
   {
-    int* sexp = reinterpret_cast<int*>(w + round_up(3 * Mp * Kp * 2, 256) + round_up(3 * Np * Kp * 2, 256));
     ptk_status ss;
     if ((ss = stage_operand(A, sa0, sa1, M, K, 3, Abf, Kp, Mp, exact, sexp, st)) != PTK_OK) return ss;
     if ((ss = stage_operand(B, sb1, sb0, N, K, 3, Bbf, Kp, Np, exact, sexp + M, st)) != PTK_OK) return ss;  // B[K,N] -> Bt[N,K]
@@ -800,6 +896,8 @@ ptk_status gemm_tc_split(int64_t M, int64_t N, int64_t K, float alpha, const flo
   p.terms = terms; p.a_rows = (int)Mp; p.b_rows = (int)Np;
   p.exact_main = exact;
   p.kchunk = split_kchunk(K, exact);
+  p.fa = reinterpret_cast<const unsigned int*>(sexp); p.fb = reinterpret_cast<const unsigned int*>(sexp + M); p.fc = nullptr;
+  p.As = Abf; p.Bs = Bbf; p.lda = Kp; p.ldb = Kp;
   return launch_gemm(ta, tb, p, st);
 }
 
@@ -847,9 +945,10 @@ extern "C" ptk_status ptk_stage_operand(const void* src_f32, int64_t sr, int64_t
   PTK_REQUIRE_INIT();
   if (src_f32 == nullptr || dst == nullptr) return ptk::fail(PTK_ERR_ARG, "ptk_stage_operand: null pointer");
   int* sexp = nullptr;
-  if (aligned) {
-    if (pieces != 3 || ld != (cols + 7) / 8 * 8 || piece_rows != (rows + 255) / 256 * 256)
-      return ptk::fail(PTK_ERR_ARG, "ptk_stage_operand: aligned staging uses the default pitch / piece pitch of ptk_stage_bytes");
+  const bool default_pitch = ld == (cols + 7) / 8 * 8 && piece_rows == (rows + 255) / 256 * 256;
+  if (aligned && (pieces != 3 || !default_pitch))
+    return ptk::fail(PTK_ERR_ARG, "ptk_stage_operand: aligned staging uses the default pitch / piece pitch of ptk_stage_bytes");
+  if (pieces == 3 && default_pitch) {   // the row words behind the pieces: row maxima / ±inf row flags
     const size_t mats = (size_t)(3 * piece_rows) * (size_t)ld * 2;
     sexp = reinterpret_cast<int*>((char*)dst + (mats + 255) / 256 * 256);
   }
@@ -861,12 +960,14 @@ extern "C" ptk_status ptk_gemm_tc_staged(int64_t M, int64_t N, int64_t K, double
                                          int64_t a_rows, const void* B_stage, int64_t ldb, int64_t b_rows, int terms,
                                          double beta, void* C, int64_t sc0, int64_t sc1, const void* bias, int act,
                                          void* C_stage, int64_t ldc_stage, int64_t c_rows, int out_pieces, int exact_main,
-                                         int out_exp, void* stream) {
+                                         int out_exp, const void* a_flags, const void* b_flags, void* c_flags,
+                                         void* stream) {
   PTK_REQUIRE_INIT();
   if (A_stage == nullptr || B_stage == nullptr || C == nullptr) return ptk::fail(PTK_ERR_ARG, "ptk_gemm_tc_staged: null operand");
   return ptk::gemm_tc_staged(M, N, K, (float)alpha, A_stage, lda, a_rows, B_stage, ldb, b_rows, terms, (float)beta, (float*)C,
                              sc0, sc1, (const float*)bias, act, C_stage, ldc_stage, c_rows, out_pieces, exact_main,
-                             out_exp == PTK_STAGE_NO_EXP ? PTK_NO_EXP : out_exp, (cudaStream_t)stream);
+                             out_exp == PTK_STAGE_NO_EXP ? PTK_NO_EXP : out_exp, (const unsigned int*)a_flags,
+                             (const unsigned int*)b_flags, (unsigned int*)c_flags, (cudaStream_t)stream);
 }
 
 extern "C" int ptk_gemm_exact_main_default(void) { return ptk::exact_main_default(); }

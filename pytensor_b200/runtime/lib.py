@@ -96,7 +96,7 @@ SIGNATURES = {
                                   c_void_p]),
     "ptk_gemm_tc_staged": (c_int, [c_int64, c_int64, c_int64, c_double, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64,
                                    c_int, c_double, c_void_p, c_int64, c_int64, c_void_p, c_int, c_void_p, c_int64, c_int64,
-                                   c_int, c_int, c_int, c_void_p]),
+                                   c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "ptk_gemm_exact_main_default": (c_int, []),
     "ptk_gemm_lead_bits": (c_int, [c_int64]),
     "ptk_mlp_chain": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int, POINTER(c_void_p), POINTER(c_void_p),

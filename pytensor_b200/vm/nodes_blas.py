@@ -130,18 +130,19 @@ class Staged:
     """A matrix in the tensor-core kernel's operand layout: `pieces` (1 = bf16, 3 = bf16x3 split) K-major matrices
     [rows, cols] stacked with a pitch of `piece_rows` rows in one device buffer."""
 
-    __slots__ = ("buf", "rows", "cols", "ld", "piece_rows", "pieces", "in_graph", "aligned")
+    __slots__ = ("buf", "rows", "cols", "ld", "piece_rows", "pieces", "in_graph", "aligned", "flagged")
 
     @classmethod
     def wrap(cls, t: torch.Tensor, rows, cols):
         """A caller-provided row-major bf16 matrix (pitch multiple of 8, 16-byte aligned) as a one-piece operand."""
         st = cls.__new__(cls)
         st.rows, st.cols, st.pieces, st.ld, st.piece_rows, st.buf, st.in_graph = int(rows), int(cols), 1, int(t.stride(0)), 0, t, False
-        st.aligned = False
+        st.aligned = st.flagged = False
         return st
 
     def __init__(self, rows, cols, pieces, aligned=False):
         self.in_graph = False
+        self.flagged = False   # the ±inf row flags behind the pieces are valid (see flags_ptr)
         self.aligned = bool(aligned) and int(pieces) == 3   # leading piece on a per-row power-of-two grid (exact main term)
         self.rows, self.cols, self.pieces = int(rows), int(cols), int(pieces)
         self.ld = (self.cols + 7) // 8 * 8
@@ -154,6 +155,11 @@ class Staged:
         if self.buf.dtype != torch.uint8:   # a caller-provided bf16 matrix used as is (already 16-byte aligned)
             return dev.ptr(self.buf)
         return (dev.ptr(self.buf) + 255) & ~255
+
+    @property
+    def flags_ptr(self):
+        """One word per row behind the three pieces (include/ptk.h): 0x7f800000 marks a row that holds ±inf."""
+        return self.ptr + (3 * self.piece_rows * self.ld * 2 + 255) // 256 * 256
 
 
 def exact_main() -> bool:
@@ -171,6 +177,7 @@ def stage_operand(t: torch.Tensor, pieces: int, transposed: bool = False, aligne
     st = Staged(R, C, pieces, aligned)
     _lib.check(_lib.lib().ptk_stage_operand(dev.ptr(t), sr, sc, R, C, pieces, 1 if st.aligned else 0, st.ptr, st.ld,
                                             st.piece_rows, dev.stream_ptr()), "ptk_stage_operand")
+    st.flagged = st.pieces == 3
     return st
 
 
@@ -205,12 +212,21 @@ def gemm_staged(A: Staged, B: Staged, terms, alpha, beta, C, bias=None, act=0, o
         if act != 1:
             raise ValueError("gemm_staged: an aligned three-piece output needs a bounded activation (tanh)")
         out_exp = int(_lib.lib().ptk_gemm_lead_bits(N)) - 1   # the result is the A operand of a contraction over N
+    c_flags = None
+    if out is not None:
+        # a tanh output (aligned) is finite or NaN and needs no flags; otherwise the epilogue raises them in zeroed words
+        out.flagged = out.pieces == 3 and not out.aligned
+        if out.flagged:
+            c_flags = out.flags_ptr
+            _lib.check(_lib.lib().ptk_memset_async(c_flags, 0, 4 * out.rows, dev.stream_ptr()), "memset")
     _lib.check(_lib.lib().ptk_gemm_tc_staged(M, N, K, float(alpha), A.ptr, A.ld, A.piece_rows, B.ptr, B.ld, B.piece_rows,
                                              int(terms), float(beta), dev.ptr(C), C.stride(0), C.stride(1),
                                              dev.ptr(bias) if bias is not None else None, int(act),
                                              out.ptr if out is not None else None, out.ld if out is not None else 0,
                                              out.piece_rows if out is not None else 0, out.pieces if out is not None else 1,
-                                             exact, out_exp, dev.stream_ptr()), "ptk_gemm_tc_staged")
+                                             exact, out_exp, A.flags_ptr if A.flagged else None,
+                                             B.flags_ptr if B.flagged else None, c_flags, dev.stream_ptr()),
+               "ptk_gemm_tc_staged")
 
 
 # ---- staged weights stay resident ---------------------------------------------------------------------------------------

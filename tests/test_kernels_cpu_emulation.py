@@ -1269,3 +1269,70 @@ def test_plain_bf16_staging_kernels(tmp_path, R, Cc, row_major):
     np.testing.assert_array_equal(p[2], _bf16_round((r1.astype(np.float64) - p[1]).astype(np.float32)))
     assert np.all(np.abs(p[0] + p[1] + p[2] - x64) <= np.abs(x64) * 2.0 ** -22)
     assert not dst[R:pr].any() and not dst[pr + R:2 * pr].any()     # rows between the pieces stay untouched
+
+
+def _special_rows(R, Cc, rng):
+    """Finite normal values except: ±inf next to zeros, tiny and normal values (row 0), NaN (row 1), a row whose largest
+    magnitude lies in the top binade above 127.5 * 2^121 (row 2), fp32 denormals (row 3), -inf alone (row 4)."""
+    x = rng.standard_normal((R, Cc)).astype(np.float32)
+    x[0, :6] = [np.inf, 0.0, 1e-3, -1e-3, -np.inf, 2.0]
+    x[1, 3] = np.nan
+    x[2, :] = (rng.uniform(-1, 1, Cc) * 3.0e38).astype(np.float32)
+    x[2, 1] = np.float32(3.40e38)          # (rounds to inf in bf16)
+    x[3, :] = (rng.standard_normal(Cc) * 1e-40).astype(np.float32)
+    x[4, :] = 0.0
+    x[4, Cc - 1] = -np.inf
+    return x
+
+
+@pytest.mark.parametrize("aligned", [False, True])
+@pytest.mark.parametrize("R,Cc,row_major", [(70, 130, True), (9, 67, False)])
+def test_three_piece_splits_of_non_finite_and_extreme_values(tmp_path, R, Cc, row_major, aligned):
+    """Both three-piece splits (split_bf16x3_kernel, split_aligned_kernel): a non-finite x is staged as (x, 0, 0) — a NaN
+    remainder would turn every piece product into NaN — and every finite x, the top binade and denormals included, as
+    finite pieces summing to x.  The row maxima row_absmax_kernel leaves (ptk_stage_operand runs it for either split) are
+    +inf exactly for the rows holding ±inf: the flags that make the GEMM recompute those rows' outputs."""
+    rng = np.random.default_rng(R + Cc)
+    x = _special_rows(R, Cc, rng)
+    src = np.ascontiguousarray(x if row_major else x.T)
+    sr, sc = (Cc, 1) if row_major else (1, R)
+    ld, pr = (Cc + 7) // 8 * 8, (R + 255) // 256 * 256
+    grid = ((Cc + 63) // 64, (R + 63) // 64)
+    cu = os.path.join(CSRC, "ptk_gemm_tc.cu")
+    text = open(cu).read()
+    dst = np.zeros((3 * pr, ld), dtype=np.uint16)
+    flags = np.zeros(R, dtype=np.uint32)
+    (tmp_path / "m").mkdir(), (tmp_path / "s").mkdir()
+    k1 = EmulatedKernel(BF16_SHIM + ATOMIC_SHIM + extract_static_kernel(cu, "row_absmax_kernel"), "row_absmax_kernel",
+                        tmp_path / "m", threaded=True)
+    k1.launch(grid, 256, [_ptr(src), c_longlong(sr), c_longlong(sc), c_longlong(R), c_longlong(Cc), _ptr(flags)])
+    if aligned:
+        i0 = text.index("__device__ __forceinline__ int scale_exp_of")
+        helper = text[i0:text.index("\n}\n", i0) + 3]
+        k2 = EmulatedKernel(BF16_SHIM + ATOMIC_SHIM + helper + extract_static_kernel(cu, "split_aligned_kernel"),
+                            "split_aligned_kernel", tmp_path / "s", threaded=True)
+        k2.launch(grid, 256, [_ptr(src), c_longlong(sr), c_longlong(sc), _ptr(dst), c_longlong(ld), c_longlong(R),
+                              c_longlong(Cc), c_longlong(pr), _ptr(flags), c_int(7)])
+    else:
+        ks = EmulatedKernel(BF16_SHIM + BF16_PAIR_SHIM + extract_static_kernel(cu, "split_bf16x3_kernel"),
+                            "split_bf16x3_kernel", tmp_path / "s", threaded=True)
+        ks.launch(grid, 256, [_ptr(src), c_longlong(sr), c_longlong(sc), _ptr(dst), c_longlong(ld), c_longlong(R),
+                              c_longlong(Cc), c_longlong(pr)])
+    has_inf = np.isinf(x).any(axis=1)
+    np.testing.assert_array_equal(flags == 0x7F800000, has_inf)
+    p = [(dst[k * pr:k * pr + R, :Cc].astype(np.uint32) << 16).view(np.float32).astype(np.float64) for k in range(3)]
+    x64 = x.astype(np.float64)
+    fin = np.isfinite(x)
+    np.testing.assert_array_equal(p[0][~fin], x64[~fin])               # inf keeps its sign, NaN stays NaN
+    assert not p[1][~fin].any() and not p[2][~fin].any()
+    assert all(np.isfinite(q[fin]).all() for q in p)
+    err = np.abs((p[0] + p[1] + p[2])[fin] - x64[fin])
+    if aligned:
+        # finite rows: 2^-23 of the row maximum; a row holding ±inf has no scale (unit 1): the remainder |x - rint(x)| <= 1/2
+        # carries 16 bits through the two correction pieces
+        rowmax = np.abs(np.where(fin, x64, 0.0)).max(axis=1)
+        bound = np.where(has_inf, 2.0 ** -17, rowmax * 2.0 ** -23)[:, None] * np.ones_like(x64)
+        bound = np.maximum(bound, 2.0 ** -134)[fin]
+    else:
+        bound = np.maximum(np.abs(x64) * 2.0 ** -22, 2.0 ** -134)[fin]   # (bf16 denormals end at 2^-133)
+    assert np.all(err <= bound), (err - bound).max()
