@@ -373,6 +373,13 @@ __device__ __forceinline__ void ptk_bulk_g2s(void* dst, const void* src, unsigne
 """
 
 TMA_STAGES = 4
+STATIC_SMEM_LIMIT = 48 * 1024   # statically declared __shared__ bytes a kernel may use
+
+
+def tma_smem_bytes(n_vec: int) -> int:
+    """Shared memory of gen_row_kernel_tma with `n_vec` streamed inputs: a ring of TMA_STAGES trips of 256 16-byte vectors
+    per input, plus the full / empty mbarriers."""
+    return n_vec * TMA_STAGES * 256 * 16 + 2 * TMA_STAGES * 8
 
 
 def _k3_tma_min_blocks() -> int:
@@ -389,7 +396,8 @@ def gen_row_kernel_tma(prog: ScalarProgram, name: str, col_modes: tuple, store_m
     (one mbarrier arrival per warp) and run the scalar bodies.  No load instruction, no address arithmetic and no register
     is spent on the prefetch, so occupancy stays that of the plain kernel while the memory system always has
     TMA_STAGES - 1 trips in flight per CTA.  Same parameters / launch geometry as gen_row_kernel; requires every
-    vector-mode input to have 16-byte vectors (vw * itemsize == 16) — the launcher falls back otherwise."""
+    vector-mode input to have 16-byte vectors (vw * itemsize == 16) and the ring to fit the static shared memory
+    (tma_smem_bytes: at most two such inputs) — the launcher uses gen_row_kernel otherwise."""
     from .scalar import ITEMSIZE
 
     n_in, n_map = len(prog.in_dtypes), len(prog.out_dtypes)

@@ -621,9 +621,11 @@ class ElemwiseReduceNode(Node):
             return self._unfused_given(vals, ins, outs)
         store = tuple((k != 0 or self.store_reduced_input) for k in range(ew.n_out))  # in self.order numbering
         in_modes = tuple(col_modes[: len(ins)])
-        # TMA staging (cp.async.bulk through shared memory) needs 16-byte vectors on every streamed input
+        # TMA staging (cp.async.bulk through shared memory) needs 16-byte vectors on every streamed input and a staging
+        # ring that fits the static shared memory
         tma = (cg_red._k3_pipeline() == "tma" and tpr >= 64
-               and all(vw * ITEMSIZE[dt] == 16 for dt, m in zip(ew.prog.in_dtypes, in_modes) if m == 1))
+               and all(vw * ITEMSIZE[dt] == 16 for dt, m in zip(ew.prog.in_dtypes, in_modes) if m == 1)
+               and cg_red.tma_smem_bytes(in_modes.count(1)) <= cg_red.STATIC_SMEM_LIMIT)
         key = (in_modes, vw, tpr, store, tma)
         fn = self._kernels.get(key)
         if fn is None:

@@ -222,6 +222,63 @@ def test_fused_map_row_reduce_kernel_k3(tmp_path, rows, cols, tpr, vw, store, tm
     np.testing.assert_allclose(r, expect.astype(np.float64).sum(axis=1).astype(np.float32), rtol=3e-6, atol=1e-6)
 
 
+K3_SCHEMES = {"none": {}, "l2": {"PTK_K3_PIPE": "l2"}, "regs": {"PTK_K3_PIPE": "regs"}, "tma": {"PTK_K3_PIPE": "tma"},
+              "idx": {"PTK_K3_ADDR": "idx"}}
+_k3_scheme_kernels = {}
+
+
+@pytest.mark.parametrize("layout", ["no_full_vector", "one_leftover_vector", "tail"])
+@pytest.mark.parametrize("scheme,tpr", [(s, t) for s in K3_SCHEMES for t in (32, 64, 128, 256)
+                                        if not (s == "tma" and t < 64)])   # (the launcher stages from 64 threads per row)
+def test_fused_map_row_reduce_load_schemes_on_the_integer_grid(tmp_path_factory, monkeypatch, scheme, tpr, layout):
+    """Every load scheme of the row kernel (PTK_K3_PIPE / PTK_K3_ADDR) at every TPR, bit for bit: integer-valued inputs
+    make the map a * s + c exact and its fp64 row sum exact, and an adjacent +G pair and -G pair per row (G + G > 2^24)
+    breaks any fp32 step in the accumulation.  Two CTAs stride over four row blocks (the register pipeline pre-loads the
+    first trip of a thread's next row), the last block is partial; cols give no full vector, one vector left over after
+    the two-vector trips, or a scalar tail behind an uneven share of vectors."""
+    G = 3 << 22
+    for v in ("PTK_K3_PIPE", "PTK_K3_ADDR", "PTK_K3_MINB"):
+        monkeypatch.delenv(v, raising=False)
+    for k, v in K3_SCHEMES[scheme].items():
+        monkeypatch.setenv(k, v)
+    dt, vw, rpb = "float32", 4, 256 // tpr
+    key = (scheme, tpr)
+    if key not in _k3_scheme_kernels:
+        prog = ScalarProgram(in_dtypes=[dt, dt, dt], out_dtypes=[dt])
+        prog.insts = [ScalarInst("Mul", [("i", 0), ("i", 1)], [dt, dt], dt), ScalarInst("Add", [("t", 0), ("i", 2)], [dt, dt], dt)]
+        prog.outputs = [("t", 1)]
+        gen = cg_red.gen_row_kernel_tma if scheme == "tma" else cg_red.gen_row_kernel
+        src = gen(prog, "k_row_s", (1, 0, 1), (True,), "add", "float64", "float32", 0, vw, tpr)
+        _k3_scheme_kernels[key] = EmulatedKernel(src, "k_row_s", tmp_path_factory.mktemp(f"k3_{scheme}_{tpr}"), threaded=True,
+                                                 warp_shim=scheme == "tma")
+    k = _k3_scheme_kernels[key]
+    ncv, tail = {"no_full_vector": (0, 3), "one_leftover_vector": (2 * tpr + 1, 0), "tail": (3 * tpr + 5, 2)}[layout]
+    cols = ncv * vw + tail
+    pitch = cols + (-cols) % vw + vw          # aligned row pitch with padding that must stay untouched
+    rows = 3 * rpb + 1
+    rng = np.random.default_rng(tpr + ncv)
+    a, c, e = _aligned((rows, pitch), dt), _aligned((rows, pitch), dt), _aligned((rows, pitch), dt)
+    s = _aligned((rows,), dt)
+    ai, ci = rng.integers(-8, 9, (rows, cols)), rng.integers(-8, 9, (rows, cols))
+    si = rng.integers(-4, 5, rows)
+    if cols >= 8:
+        m = cols // 2 - 1
+        p1 = rng.integers(0, m, rows)
+        p2 = (p1 + rng.integers(1, m, rows)) % m
+        for p, v in ((p1, G), (p2, -G)):
+            ci[np.arange(rows), 2 * p] = ci[np.arange(rows), 2 * p + 1] = v
+    a[:, :cols], c[:, :cols], s[:] = ai, ci, si
+    e[...] = 12345.0
+    r = _aligned((rows,), dt)
+    args = [_ptr(a), _ptr(s), _ptr(c), _ptr(e), _ptr(r), c_longlong(pitch), c_longlong(1), c_longlong(pitch), c_longlong(pitch),
+            c_longlong(rows), c_longlong(cols), c_int(1)]
+    k.launch((2, 1), 256, args)
+    exact = ai * si[:, None] + ci
+    np.testing.assert_array_equal(e[:, :cols], exact.astype(dt))
+    assert np.all(e[:, cols:] == 12345.0)
+    np.testing.assert_array_equal(r, exact.sum(axis=1).astype(np.float64).astype(dt))
+
+
 @pytest.mark.parametrize("red_op,np_fn,identity", [("add", np.sum, 0), ("maximum", np.max, float("-inf")), ("mul", np.prod, 1)])
 def test_column_and_generic_reduce_kernels(tmp_path, red_op, np_fn, identity):
     rng = np.random.default_rng(7)
