@@ -146,6 +146,21 @@ ptk_status   ptk_cumop(int dtype, int op, const void* x, void* out, int64_t oute
  * sequential): parity with the reference is distributional. */
 ptk_status   ptk_random_fill(int dist, int dtype, void* out, int64_t n, uint64_t key, uint64_t seed, const void* p0, int64_t s0,
                              const void* p1, int64_t s1, const void* p2, int64_t s2, void* stream);
+/* Discrete counts, with the parameter walk of ptk_random_fill: dist 0 poisson(lam), 1 binomial(n, p),
+ * 2 negative_binomial(n, p) (= poisson(gamma(n) * (1-p)/p)), 3 geometric(p) (support from 1), 4 beta_binomial(n, a, b).
+ * Stream = element index.  An element whose parameters NumPy / SciPy reject (e.g. lam < 0, p outside [0, 1], a
+ * non-integer beta-binomial n, an n above 2^53, NumPy's "n too large or p too small") sets the device int word *err to 1 and
+ * draws 0; *err is never cleared here.  dtype: any integer, bool or float type (int64 draws saturate at 2^63 - 1). */
+ptk_status   ptk_random_count(int dist, int dtype, void* out, int64_t n, uint64_t key, uint64_t seed, const void* p0, int64_t s0,
+                              const void* p1, int64_t s1, const void* p2, int64_t s2, int* err, void* stream);
+/* Row samplers over `rows` batch rows of k contiguous float64 parameters, row r at p + r*ps (ps = 0: one row for all, k: one
+ * per row).  kind 0 categorical(p): out[rows] = searchsorted(cumsum(p[r]), u, side="left") (k when u exceeds the total; p is
+ * not validated), stream = row.  kind 1 multinomial(n, p): out[rows, k], n = nv[r * ns] (ns 0 or 1), conditional
+ * binomials over 0..k-2 and the remainder in k-1, stream = row; n < 0 or above 2^53, a p outside [0, 1] or NaN, or
+ * sum(p[:-1]) > 1 + 1e-12 set *err.  kind 2 dirichlet(alpha = p): out[rows, k] float, stream = r*k + j for component j;
+ * alpha < 0 sets *err, alpha = 0 gives 0, a NaN alpha a NaN row. */
+ptk_status   ptk_random_rows(int kind, int dtype, void* out, int64_t rows, int64_t k, uint64_t key, uint64_t seed, const void* p,
+                             int64_t ps, const void* nv, int64_t ns, int* err, void* stream);
 
 /* ---- BLAS family (A5/A6: Gemm tensor/blas/gemm.py:76, Dot22 :248, Dot22Scalar :298, Gemv tensor/blas/gemv.py:16,
  *      Ger tensor/blas/ger.py:8; the C linker calls sgemm_/dgemm_/sgemv_/dgemv_ at blas/c_code/codegen.py:463-805) */

@@ -156,8 +156,9 @@ class CudaVM:
         return res
 
     def check_errors(self):
-        """Synchronise and raise the IndexError an earlier device-output / updates-only call may have flagged (those
-        calls never synchronise themselves; the next call of this function would raise it too)."""
+        """Synchronise and raise the error (IndexError, or ValueError for a rejected sampler parameter) that an earlier
+        device-output / updates-only call may have flagged (those calls never synchronise themselves; the next call of
+        this function would raise it too)."""
         self.executor.sink.check(sync=True)
 
     def clear_storage(self):

@@ -316,14 +316,19 @@ def lower_node(node, opts):
     from pytensor.tensor.random.op import RandomVariable
 
     if isinstance(op, RandomVariable):
-        from pytensor_b200.vm.nodes_random import DIST, RandomVariableNode
+        from pytensor_b200.vm.nodes_random import COUNT, DIST, ROWS, RandomRowsNode, RandomVariableNode
         from pytensor.tensor.type_other import NoneTypeT
 
-        if op.name not in DIST or op.ndim_supp != 0 or len(node.inputs) - 2 != DIST[op.name][1]:
-            raise UnsupportedOp(f"{op}: random variable '{op.name}' has no device sampler (supported: {sorted(DIST)})")
+        table = {**DIST, **COUNT, **ROWS}
+        supp = 1 if op.name in ("multinomial", "dirichlet") else 0
+        if op.name not in table or op.ndim_supp != supp or len(node.inputs) - 2 != table[op.name][1]:
+            raise UnsupportedOp(f"{op}: random variable '{op.name}' has no device sampler (supported: {sorted(table)})")
         if op.dtype not in ("float32", "float64", "int64", "int32", "int16", "int8", "uint8", "bool"):
             raise UnsupportedOp(f"{op}: draws of dtype {op.dtype}")
-        return RandomVariableNode(op.name, op.dtype, bool(op.inplace), isinstance(node.inputs[1].type, NoneTypeT), name=str(op))
+        size_is_none = isinstance(node.inputs[1].type, NoneTypeT)
+        if op.name in ROWS:
+            return RandomRowsNode(op.name, op.dtype, bool(op.inplace), size_is_none, name=str(op))
+        return RandomVariableNode(op.name, op.dtype, bool(op.inplace), size_is_none, name=str(op))
 
     if cname == "BatchedDot":
         dt = node.outputs[0].type.dtype

@@ -76,6 +76,10 @@ SIGNATURES = {
     "ptk_nonzero_fill": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "ptk_random_fill": (c_int, [c_int, c_int, c_void_p, c_int64, ctypes.c_uint64, ctypes.c_uint64, c_void_p, c_int64, c_void_p,
                                 c_int64, c_void_p, c_int64, c_void_p]),
+    "ptk_random_count": (c_int, [c_int, c_int, c_void_p, c_int64, ctypes.c_uint64, ctypes.c_uint64, c_void_p, c_int64,
+                                 c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p]),
+    "ptk_random_rows": (c_int, [c_int, c_int, c_void_p, c_int64, c_int64, ctypes.c_uint64, ctypes.c_uint64, c_void_p, c_int64,
+                                c_void_p, c_int64, c_void_p, c_void_p]),
     "ptk_arange": (c_int, [c_int, c_void_p, c_int64, c_double, c_double, c_int64, c_int64, c_void_p]),
     "ptk_argmax": (c_int, [c_int, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
     "ptk_cumop": (c_int, [c_int, c_int, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),

@@ -442,7 +442,7 @@ class FlagSink:
     def __init__(self):
         self.words = None     # device int32[SLOTS]
         self.mirror = None    # pinned host int32[SLOTS]
-        self.msgs = [None] * self.SLOTS
+        self.msgs = [None] * self.SLOTS   # (message, exception class) of each slot
         self.cursor = 0
         self.used = False     # some launch of the current call took a slot
         self.in_flight = False
@@ -467,12 +467,13 @@ class FlagSink:
         self.cursor = 0
         self.used = False
 
-    def slot(self, msg) -> int:
-        """Device address of the next error word of this call (program order -> the same slot on every call)."""
+    def slot(self, msg, exc=IndexError) -> int:
+        """Device address of the next error word of this call (program order -> the same slot on every call); a flagged
+        word raises `exc(msg)`."""
         self._ensure()
         k = min(self.cursor, self.SLOTS - 1)
         self.cursor += 1
-        self.msgs[k] = msg if self.cursor <= self.SLOTS else "index out of bounds"
+        self.msgs[k] = (msg, exc) if self.cursor <= self.SLOTS or exc is not IndexError else ("index out of bounds", exc)
         self.used = True
         return dev.ptr(self.words) + 4 * k
 
@@ -485,7 +486,8 @@ class FlagSink:
         self.in_flight = True
 
     def check(self, sync=False):
-        """Raise IndexError (like the reference's C code) if a completed call flagged an out-of-bounds index."""
+        """Raise the exception of the first flagged slot (IndexError for an out-of-bounds index, like the reference's C
+        code; ValueError for a parameter a random sampler rejects) if a completed call flagged one."""
         if self.words is None or not self.in_flight:
             return
         if sync:
@@ -494,10 +496,10 @@ class FlagSink:
             dev.synchronize()
         bad = np.flatnonzero(self.mirror)
         if bad.size:
-            msg = self.msgs[int(bad[0])] or "index out of bounds"
+            msg, exc = self.msgs[int(bad[0])] or ("index out of bounds", IndexError)
             self.mirror[:] = 0
             _lib.check(_lib.lib().ptk_memset_async(dev.ptr(self.words), 0, 4 * self.SLOTS, dev.stream_ptr()), "memset")
-            raise IndexError(msg)
+            raise exc(msg)
         if sync:
             self.in_flight = False
 
@@ -510,9 +512,9 @@ def current_sink() -> FlagSink:
     return _sink_stack[-1] if _sink_stack else _default_sink
 
 
-def _err_flag(msg="index out of bounds") -> int:
+def _err_flag(msg="index out of bounds", exc=IndexError) -> int:
     """Device ADDRESS (int) of an error word owned by the running Executor."""
-    return current_sink().slot(msg)
+    return current_sink().slot(msg, exc)
 
 
 def check_pending_flags():
