@@ -314,11 +314,18 @@ OPS = {
     "GammaInc": lambda a, it, ot: f"ptk_gamma_p((double)({a[0]}), (double)({a[1]}))",
     "GammaIncC": lambda a, it, ot: f"ptk_gamma_q((double)({a[0]}), (double)({a[1]}))",
     "BetaInc": lambda a, it, ot: f"ptk_betainc((double)({a[0]}), (double)({a[1]}), (double)({a[2]}))",
+    # the reference evaluates these four through SciPy (scalar/math.py PolyGamma, GammaIncInv, GammaIncCInv, BetaIncInv
+    # have no C code), in double whatever the graph dtype
+    "PolyGamma": lambda a, it, ot: f"ptk_polygamma((long long)({a[0]}), (double)({a[1]}))",
+    "GammaIncInv": lambda a, it, ot: f"ptk_gammaincinv((double)({a[0]}), (double)({a[1]}))",
+    "GammaIncCInv": lambda a, it, ot: f"ptk_gammainccinv((double)({a[0]}), (double)({a[1]}))",
+    "BetaIncInv": lambda a, it, ot: f"ptk_betaincinv((double)({a[0]}), (double)({a[1]}), (double)({a[2]}))",
 }
 
 # which helper blocks (SPECIAL_HELPERS) an op's expression needs
 NEEDS = {"Psi": ("psi",), "TriGamma": ("trigamma",), "GammaInc": ("gammainc",), "GammaIncC": ("gammainc",),
-         "BetaInc": ("betainc",)}
+         "BetaInc": ("betainc",), "PolyGamma": ("polygamma",), "GammaIncInv": ("gammainc", "gammaincinv"),
+         "GammaIncCInv": ("gammainc", "gammaincinv"), "BetaIncInv": ("betainc", "betaincinv")}
 
 
 # Device restatements of the reference's double-precision special functions.  Emitted in front of a scalar body only when
@@ -497,6 +504,267 @@ __device__ inline double ptk_betainc(double a, double b, double x) {
   }
   if (flipped) return t <= eps ? 1.0 - eps : 1.0 - t;
   return t;
+}
+#endif
+""",
+    # PolyGamma(n, x), SciPy's definition: digamma for n = 0, (-1)^(n+1) n! zeta(n+1, x) for n >= 1, NaN for n < 0.
+    # Digamma: reflection psi(x) = psi(1-x) - pi cot(pi x) for x < 0 (-inf at +0, +inf at -0, NaN at negative
+    # integers), a Taylor series about the positive root x0 = 1.4616... within 0.1 of it (so the result keeps its
+    # relative accuracy where it crosses zero), else the recurrence up to 10 and the asymptotic series.
+    # Hurwitz zeta: Euler-Maclaurin summation.  Direct terms (q+k)^-s until q+k >= 10+s or they stop contributing, then
+    # the integral, half-term and 12 Bernoulli corrections; +inf at non-positive integer q (and -inf), as in SciPy.
+    # Trip caps: the direct sum stops after 256 terms (NaN when q + 256 is still below 10+s: non-integer q < -230 for
+    # small n), the Bernoulli loop after 12; digamma's recurrence runs at most 10 times.  The product form keeps SciPy's
+    # overflow (n! = inf from n = 171) and 0 * inf = NaN (zeta underflowing for large n and x).
+    "polygamma": r"""
+#ifndef PTK_HAVE_POLYGAMMA
+#define PTK_HAVE_POLYGAMMA
+__device__ inline double ptk_digamma(double x) {
+  const double inf = __longlong_as_double(0x7ff0000000000000LL), pi = 3.14159265358979323846;
+  if (isnan(x)) return x;
+  if (x == 0.0) return signbit(x) ? inf : -inf;
+  double acc = 0.0;
+  if (x < 0.0) {
+    if (x == floor(x)) return __longlong_as_double(0x7ff8000000000000LL);
+    acc = -pi * cospi(x) / sinpi(x);
+    x = 1.0 - x;
+  }
+  const double h = (x - 1.4616321449683622) - 9.549995429965697e-17;
+  if (fabs(h) < 0.1) {
+    const double c[14] = {0.9676722454476212, -0.4427631689835921, 0.258499760955651, -0.16394270544240652,
+                          0.10782405069126237, -0.07219956125645471, 0.04880428816414311, -0.03316112647484736,
+                          0.022597648232218104, -0.01542476590494896, 0.010538791616612175, -0.007204534386356869,
+                          0.004926781395729853, -0.003369801655439328};
+    double s = c[13];
+    for (int k = 12; k >= 0; --k) s = s * h + c[k];
+    return s * h + acc;
+  }
+  double s = 0.0;
+  for (int k = 0; k < 10 && x < 10.0; ++k) { s -= 1.0 / x; x += 1.0; }
+  const double r2 = 1.0 / (x * x);
+  const double t = r2 * (0.08333333333333333 + r2 * (-0.008333333333333333 + r2 * (0.003968253968253968 +
+                   r2 * (-0.004166666666666667 + r2 * (0.007575757575757576 + r2 * (-0.021092796092796094 +
+                   r2 * 0.08333333333333333))))));
+  return (s + (log(x) - 0.5 / x - t)) + acc;
+}
+// zeta(s, q) = sum_{k >= 0} (q + k)^-s for s >= 2
+__device__ inline double ptk_hurwitz_zeta(double s, double q) {
+  const double eps = 1.1102230246251565e-16;
+  if (isnan(q)) return q;
+  if (q <= 0.0 && q == floor(q)) return __longlong_as_double(0x7ff0000000000000LL);
+  if (isinf(q)) return 0.0;
+  const double W = 10.0 + s;
+  double sum = 0.0, w = q;
+  for (int k = 0; k < 256 && w < W; ++k) {
+    const double t = pow(w, -s);
+    sum += t;
+    w += 1.0;
+    if (w > 1.0 && fabs(t) <= eps * fabs(sum)) return sum;
+  }
+  if (w < W) return __longlong_as_double(0x7ff8000000000000LL);
+  const double b2j[12] = {0.08333333333333333, -0.001388888888888889, 3.306878306878307e-05, -8.267195767195768e-07,
+                          2.08767569878681e-08, -5.284190138687493e-10, 1.3382536530684679e-11, -3.3896802963225827e-13,
+                          8.586062056277845e-15, -2.174868698558062e-16, 5.5090028283602295e-18, -1.3954464685812522e-19};
+  const double a = pow(w, -s);
+  sum += w * a / (s - 1.0) + 0.5 * a;
+  double f = s * a / w;  // (s)_(2j-1) w^(-s-2j+1)
+  for (int j = 0; j < 12; ++j) {
+    const double t = f * b2j[j];
+    sum += t;
+    if (fabs(t) <= eps * fabs(sum)) break;
+    f *= (s + 2.0 * j + 1.0) * (s + 2.0 * j + 2.0) / (w * w);
+  }
+  return sum;
+}
+__device__ inline double ptk_polygamma(long long n, double x) {
+  if (n == 0) return ptk_digamma(x);
+  if (n < 0) return __longlong_as_double(0x7ff8000000000000LL);
+  const double s = (double)n + 1.0;
+  return ((n & 1) ? 1.0 : -1.0) * tgamma(s) * ptk_hurwitz_zeta(s, x);
+}
+#endif
+""",
+    # Inverse regularised incomplete gamma (needs "gammainc").  One solver for both tails: it targets whichever of P and
+    # Q = 1 - P is <= 1/2 at the solution (1 - t is exact there), so neither tail loses digits to the other.  Unknown
+    # u = log x; residual g(u) = +-(log T(e^u) - log t), where log T is formed here as the log prefactor
+    # a u - x - lgamma(a) plus the log of ptk_gamma_series / ptk_gamma_cfrac, so far tails do not underflow.  Start
+    # (after DiDonato & Morris 1986, Temme 1992): (P Gamma(a+1))^(1/a) for small x; Wilson-Hilferty with the
+    # Abramowitz-Stegun 26.2.23 normal deviate for a > 1; the log-tail form x = -log(Q Gamma(a)) + (a-1) log x for
+    # the upper tail of a <= 1.  Then Halley steps in u, kept inside a bracket [lo, hi] that every evaluation narrows
+    # (a step that leaves it bisects), over u in [-745.2, 709.8].  At most 64 iterations: worst case 64 evaluations of
+    # the series or continued fraction (each capped at 1024 terms) per element.
+    "gammaincinv": r"""
+#ifndef PTK_HAVE_GAMMAINCINV
+#define PTK_HAVE_GAMMAINCINV
+// log P (which = 0) or log Q (which = 1) at x, given the log prefactor lpref = a log x - x - lgamma(a); *e gets
+// |d log T / d log x| = exp(lpref - log T), taken from the series or fraction itself where log T is lpref plus its log
+// (the difference of the two logs would cancel for large x)
+__device__ inline double ptk_gamma_logpq(double a, double x, double lpref, int which, double* e) {
+  if (x < a + 1.0) {
+    const double s = ptk_gamma_series(a, x), lp = lpref + log(s);
+    if (!which) { *e = 1.0 / s; return lp; }
+    const double lq = log1p(-exp(lp));
+    *e = exp(lpref - lq);
+    return lq;
+  }
+  const double f = ptk_gamma_cfrac(a, x), lq = lpref + log(f);
+  if (which) { *e = 1.0 / f; return lq; }
+  const double lp = log1p(-exp(lq));
+  *e = exp(lpref - lp);
+  return lp;
+}
+// Abramowitz & Stegun 26.2.23: the z > 0 with upper-tail probability t (0 < t <= 1/2), to about 4.5e-4 (a start only)
+__device__ inline double ptk_normal_deviate_start(double t) {
+  const double r = sqrt(-2.0 * log(t));
+  return r - (2.515517 + r * (0.802853 + r * 0.010328)) / (1.0 + r * (1.432788 + r * (0.189269 + r * 0.001308)));
+}
+// x with P(a, x) = t (which = 0) or Q(a, x) = t (which = 1); a finite and > 0, 0 < t < 1
+__device__ inline double ptk_gammaincinv_tail(double a, double t, int which) {
+  if (t > 0.5) { t = 1.0 - t; which ^= 1; }
+  const double lt = log(t), lga = lgamma(a), sg = which ? -1.0 : 1.0;
+  const double us = ((which ? log1p(-t) : lt) + lgamma(a + 1.0)) / a;  // P ~ x^a / Gamma(a+1) for small x
+  if (us < -745.2) return 0.0;                                          // below the smallest denormal
+  double u = us;
+  if (a > 1.0) {
+    const double z = which ? ptk_normal_deviate_start(t) : -ptk_normal_deviate_start(t);
+    const double c = 1.0 / (9.0 * a), w = 1.0 - c + z * sqrt(c);
+    if (w > 0.05) u = log(a) + 3.0 * log(w);
+  } else if (which && -lt - lga > 1.0) {
+    double x = -lt - lga;
+    x = fmax(-lt - lga + (a - 1.0) * log(x), 1.0);
+    x = fmax(-lt - lga + (a - 1.0) * log(x), 1.0);
+    u = log(x);
+  }
+  double lo = -745.2, hi = 709.8, dx = hi - lo, dold = dx;
+  u = fmin(fmax(u, lo), hi);
+  for (int it = 0; it < 64; ++it) {
+    const double x = exp(u), lpref = a * u - x - lga;
+    double e;
+    const double g = sg * (ptk_gamma_logpq(a, x, lpref, which, &e) - lt);
+    if (g == 0.0) break;
+    if (g < 0.0) lo = u; else hi = u;
+    // Halley's correction only while it is small (far from the root it is a difference of large terms)
+    const double d = g / e, hf = 0.5 * d * (a - x - sg * e), tol = 2.0e-15 * fmax(1.0, fabs(u));
+    double un = u - (fabs(hf) < 0.5 ? d / (1.0 - hf) : d);
+    const bool inside = un >= lo && un <= hi;
+    if (inside && fabs(d) <= tol) { u = un; break; }
+    // bisect when the step leaves the bracket or does not halve the step before last, unless the Newton step has
+    // stopped shrinking at the rounding noise of the forward function: then the root is found
+    if (!inside || fabs(un - u) > 0.5 * fabs(dold)) {
+      if (inside && fabs(d) < 1e-11 * fmax(1.0, fabs(u))) { u = un; break; }
+      un = 0.5 * (lo + hi);
+    }
+    dold = dx;
+    dx = un - u;
+    u = un;
+    if (hi - lo <= tol) break;
+  }
+  return exp(u);
+}
+__device__ inline double ptk_gammaincinv(double a, double p) {
+  if (!(a > 0.0) || isinf(a) || !(p >= 0.0 && p <= 1.0)) return __longlong_as_double(0x7ff8000000000000LL);
+  if (p == 0.0) return 0.0;
+  if (p == 1.0) return __longlong_as_double(0x7ff0000000000000LL);
+  return ptk_gammaincinv_tail(a, p, 0);
+}
+__device__ inline double ptk_gammainccinv(double a, double q) {
+  if (!(a > 0.0) || isinf(a) || !(q >= 0.0 && q <= 1.0)) return __longlong_as_double(0x7ff8000000000000LL);
+  if (q == 0.0) return __longlong_as_double(0x7ff0000000000000LL);
+  if (q == 1.0) return 0.0;
+  return ptk_gammaincinv_tail(a, q, 1);
+}
+#endif
+""",
+    # Inverse regularised incomplete beta (needs "betainc"), by the same scheme as "gammaincinv": the solver targets the
+    # tail <= 1/2 (I_x(a,b) = p, or I_{1-x}(b,a) = 1-p through the a<->b, x<->1-x symmetry) and iterates on the logit
+    # v = log(x / (1-x)), from which both x and 1-x follow to full relative precision.  log I is the log prefactor
+    # a log x + b log(1-x) - log B(a,b) plus the log of ptk_betainc_cf over a (x <= (a+1)/(a+b+2)), or log1p of minus
+    # the same form of I_{1-x}(b,a) (above): one formula family on both sides, so the residual has no jump where the
+    # side changes.  Start: the normal approximation of AS 109 (Cran, Martin & Thomas 1977) for a, b > 1, else
+    # x^a / (a B(a,b)) = p; then bracketed Halley steps on v in [-745.2, 745.2].  At most 64 iterations: worst case 64
+    # continued-fraction evaluations (each capped at 300 terms, no other loop) per element.  Quantiles below DBL_MIN return the largest
+    # denormal, as SciPy does in general (it returns 0 for b = 1, for a = b = 1/2 and for some denormal quantiles, see
+    # DESIGN.md section 9).
+    "betaincinv": r"""
+#ifndef PTK_HAVE_BETAINCINV
+#define PTK_HAVE_BETAINCINV
+// log I_x(a, b), with x and xc = 1 - x both given to full precision (lx, lxc their logs) and lb = log B(a, b); *e gets
+// d log I / d logit(x) = x^a (1-x)^b / (B(a,b) I).  Both sides use the same log prefactor and continued fraction:
+// I_x(a, b) itself for x <= (a+1)/(a+b+2), 1 - I_{1-x}(b, a) above.  That switch keeps each fraction where it converges
+// within its 300 terms (the mean a/(a+b) would not: at a = 4497, b = 1.2e-3 the root lies between 1 - (a+1)/(a+b+2)
+// and the mean, where I_x(a, b)'s fraction has not converged), so log I is continuous across it to rounding and never
+// passes through a linear-scale value that could overflow or underflow
+__device__ inline double ptk_betainc_log(double a, double b, double x, double xc, double lx, double lxc, double lb,
+                                         double* e) {
+  const double lp = a * lx + b * lxc - lb;  // log of x^a (1-x)^b / B(a, b)
+  if (x * (a + b + 2.0) <= a + 1.0) {
+    const double w = (x * (a + b - 2.0) - (a - 1.0) < 0.0) ? ptk_betainc_cf(a, b, x, 0) : ptk_betainc_cf(a, b, x, 1) / xc;
+    *e = a / w;
+    return lp - log(a) + log(w);
+  }
+  const double w = (xc * (a + b - 2.0) - (b - 1.0) < 0.0) ? ptk_betainc_cf(b, a, xc, 0) : ptk_betainc_cf(b, a, xc, 1) / x;
+  const double li = log1p(-exp(lp - log(b) + log(w)));
+  *e = exp(lp - li);
+  return li;
+}
+__device__ inline double ptk_betaincinv(double a, double b, double p) {
+  // (SciPy's floor for an underflowing quantile is the largest denormal, one ulp below DBL_MIN)
+  const double nan = __longlong_as_double(0x7ff8000000000000LL), largest_denormal = __longlong_as_double(0x000fffffffffffffLL);
+  if (!(a > 0.0) || !(b > 0.0) || !(p >= 0.0 && p <= 1.0)) return nan;
+  if (p == 0.0) return 0.0;
+  if (p == 1.0) return 1.0;
+  if (isinf(a)) return isinf(b) ? nan : 1.0;
+  if (isinf(b)) return 0.0;
+  int which = 0;
+  double t = p;
+  if (t > 0.5) { t = 1.0 - t; which = 1; }
+  // solve for the lower tail of (A, B) at y, where y = x (which = 0) or y = 1 - x (which = 1); v is the logit of y
+  const double A = which ? b : a, B = which ? a : b, lt = log(t);
+  // log B(a, b); with the larger parameter L >= 20, lgamma(L) - lgamma(L + s) from Stirling's series, where
+  // log1p keeps the digits lgamma's difference would cancel (s = 1e-3 next to L = 1e6)
+  const double s = fmin(a, b), L = fmax(a, b);
+  double lb = lgamma(a) + lgamma(b) - lgamma(a + b);
+  if (L >= 20.0) {
+    const double r = 1.0 / L, r2 = r * r, q = 1.0 / (L + s), q2 = q * q;
+    const double cl = r * (0.08333333333333333 - r2 * (0.002777777777777778 - r2 * (7.936507936507937e-4 - r2 * 5.952380952380952e-4)));
+    const double cq = q * (0.08333333333333333 - q2 * (0.002777777777777778 - q2 * (7.936507936507937e-4 - q2 * 5.952380952380952e-4)));
+    lb = lgamma(s) - (L - 0.5) * log1p(s / L) - s * log(L + s) + s + (cl - cq);
+  }
+  double v = (lt + log(A) + lb) / A;  // log y from y^A / (A B(A,B)) = t
+  if (!which && v < -708.3964185322641) return largest_denormal;
+  if (A > 1.0 && B > 1.0) {
+    const double r = sqrt(-2.0 * lt);
+    const double y = r - (2.30753 + 0.27061 * r) / (1.0 + (0.99229 + 0.04481 * r) * r);
+    const double h = 2.0 / (1.0 / (2.0 * A - 1.0) + 1.0 / (2.0 * B - 1.0)), lam = (y * y - 3.0) / 6.0;
+    const double w = y * sqrt(h + lam) / h - (1.0 / (2.0 * B - 1.0) - 1.0 / (2.0 * A - 1.0)) * (lam + 5.0 / 6.0 - 2.0 / (3.0 * h));
+    v = log(A / B) - 2.0 * w;
+  } else {
+    v = v - log1p(-exp(fmin(v, -1e-3)));
+  }
+  double lo = -745.2, hi = 745.2, dx = hi - lo, dold = dx;
+  v = fmin(fmax(v, lo), hi);
+  for (int it = 0; it < 64; ++it) {
+    const double y = 1.0 / (1.0 + exp(-v)), yc = 1.0 / (1.0 + exp(v));
+    const double ly = -log1p(exp(-v)), lyc = -log1p(exp(v));
+    double e;
+    const double g = ptk_betainc_log(A, B, y, yc, ly, lyc, lb, &e) - lt;
+    if (g == 0.0) break;
+    if (g < 0.0) lo = v; else hi = v;
+    const double d = g / e, hf = 0.5 * d * (A * yc - B * y - e), tol = 2.0e-15 * fmax(1.0, fabs(v));
+    double vn = v - (fabs(hf) < 0.5 ? d / (1.0 - hf) : d);
+    const bool inside = vn >= lo && vn <= hi;
+    if (inside && fabs(d) <= tol) { v = vn; break; }
+    if (!inside || fabs(vn - v) > 0.5 * fabs(dold)) {
+      if (inside && fabs(d) < 1e-11 * fmax(1.0, fabs(v))) { v = vn; break; }
+      vn = 0.5 * (lo + hi);
+    }
+    dold = dx;
+    dx = vn - v;
+    v = vn;
+    if (hi - lo <= tol) break;
+  }
+  const double x = which ? 1.0 / (1.0 + exp(v)) : 1.0 / (1.0 + exp(-v));
+  return x < largest_denormal ? largest_denormal : x;
 }
 #endif
 """,
