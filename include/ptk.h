@@ -265,6 +265,15 @@ ptk_status   ptk_potrf(int dtype, void* A, int64_t n, int64_t batch, int lower, 
  * singular (zero diagonal) -> B NaN-filled (triangular.py:68-69). */
 ptk_status   ptk_trsm(int dtype, const void* A, void* B, int64_t n, int64_t nrhs, int64_t batch,
                       int lower, int trans, int unit_diag, void* stream);
+/* Cholesky solve, LAPACK ?potrs semantics (CholeskySolve, solvers/psd.py:35-54): lower != 0 -> A = C C^T, solve C y = b then
+ * C^T x = y; lower == 0 -> A = U^T U, solve U^T y = b then U x = y.  Only the referenced triangle of each factor is read.
+ * No zero-diagonal check and no NaN-fill: a zero pivot gives IEEE inf / NaN.  B is the contiguous (batch..., n, nrhs) output,
+ * holding b broadcast to the output batch shape on entry, solved in place.  The factors are contiguous (n, n); the factor of
+ * output system i lies at C + sum_d idx_d(i) * factor_batch_strides[d] elements, idx = i decomposed row-major over
+ * batch_shape[nbatch_dims] (nbatch_dims <= 8; a stride of 0 broadcasts).  Shape and strides travel as kernel arguments, so a
+ * call can be captured into a CUDA graph.  float32 / float64. */
+ptk_status   ptk_potrs(int dtype, const void* C, void* B, int64_t n, int64_t nrhs, int lower, int nbatch_dims,
+                       const int64_t* batch_shape, const int64_t* factor_batch_strides, void* stream);
 
 /* ---- multi-GPU exchange (SURVEY.md §8e C1; no counterpart in the reference, which has no collectives) ----------------------
  * One-shot all-reduce (sum) of a small vector (n <= nmax) over NVLink peer memory.  `peer_ptrs[world]` (host array) are the

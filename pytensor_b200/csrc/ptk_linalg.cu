@@ -1,5 +1,6 @@
-// Dense factor / triangular-solve kernels for Cholesky and SolveTriangular
-// (pytensor/tensor/linalg/decomposition/cholesky.py:18 potrf :52-83; solvers/triangular.py:13 trtrs :41-71).
+// Dense factor / triangular-solve kernels for Cholesky, SolveTriangular and CholeskySolve
+// (pytensor/tensor/linalg/decomposition/cholesky.py:18 potrf :52-83; solvers/triangular.py:13 trtrs :41-71;
+// solvers/psd.py:14 potrs :35-54).
 //
 // Small matrices (n <= 128, typically batched through Blockwise): one CTA per matrix / per 32-RHS panel, warp-cooperative
 // (lanes along the dot-product index).  Large matrices: right-looking BLOCKED algorithms with 64-wide panels — a
@@ -281,11 +282,81 @@ ptk_status potrf_blocked(int dtype, T* A, int64_t n, int64_t rs, int64_t cs, int
   return PTK_OK;
 }
 
+// ---- Cholesky solve (potrs) --------------------------------------------------------------------------------------------
+// Batch layout of ptk_potrs: system i of the output is decomposed over `shape` (row-major); its factor lies at
+// sum_d idx_d * stride[d] elements from the base (stride 0 = broadcast).  Passed by value, so nothing is uploaded.
+constexpr int POTRS_MAX_DIMS = 8;
+struct PotrsBatch {
+  int nd;
+  int64_t shape[POTRS_MAX_DIMS];
+  int64_t stride[POTRS_MAX_DIMS];
+};
+
+constexpr int POTRS_WARPS = 8;      // warps per CTA of potrs_small_kernel
+constexpr int POTRS_SMALL_N = 128;  // largest n of the one-launch path
+
+// small path: A = C C^T (lower) or U^T U (upper), both triangular sweeps in one launch.  One warp per (system, RHS column);
+// the column lives in the warp's shared-memory row `x`.  Warps are independent (no block barrier) and take consecutive
+// pairs with the column index fastest, so the columns of one system read its factor through L1.  The stored triangle is
+// read by rows in every sweep: where row i holds the coefficients of unknowns already solved, lanes run along k and a
+// shuffle reduction forms the dot product; where it holds those of pending unknowns, x_i is finished first and the lanes
+// update the pending entries.  Division by the diagonal, no zero check: a zero pivot gives IEEE inf / NaN like ?potrs.
+template <typename T>
+__global__ void __launch_bounds__(POTRS_WARPS * 32) potrs_small_kernel(const T* __restrict__ C, T* __restrict__ B, int64_t n,
+                                                                       int64_t nrhs, int lower, PotrsBatch bat, int64_t npairs) {
+  __shared__ T xs[POTRS_WARPS][POTRS_SMALL_N];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T* x = xs[warp];
+  const int64_t nwarps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t p = (int64_t)blockIdx.x * (blockDim.x >> 5) + warp; p < npairs; p += nwarps) {
+    const int64_t sys = p / nrhs, col = p - sys * nrhs;
+    int64_t off = 0, rem = sys;
+    for (int d = bat.nd - 1; d >= 0; --d) {
+      const int64_t q = rem / bat.shape[d];
+      off += (rem - q * bat.shape[d]) * bat.stride[d];
+      rem = q;
+    }
+    const T* A = C + off;
+    T* b = B + sys * n * nrhs + col;
+    for (int64_t i = lane; i < n; i += 32) x[i] = b[i * nrhs];
+    __syncwarp();
+    // sweep 1 runs forward, sweep 2 backward.  lower: C y = b (dot form), C^T x = y (axpy form);
+    // upper: U^T y = b (axpy form), U x = y (dot form).
+    for (int sweep = 0; sweep < 2; ++sweep) {
+      const bool fwd = sweep == 0, dot = (sweep == 0) == (lower != 0);
+      for (int64_t step = 0; step < n; ++step) {
+        const int64_t i = fwd ? step : n - 1 - step;
+        const T* row = A + i * n;
+        if (dot) {
+          T s = T(0);
+          if (fwd) for (int64_t k = lane; k < i; k += 32) s += row[k] * x[k];
+          else     for (int64_t k = i + 1 + lane; k < n; k += 32) s += row[k] * x[k];
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+          if (lane == 0) x[i] = (x[i] - s) / row[i];
+        } else {
+          T xi = T(0);
+          if (lane == 0) xi = x[i] / row[i];
+          xi = __shfl_sync(0xffffffffu, xi, 0);  // (only lane 0 reads x[i], so its store below races with no read)
+          if (fwd) for (int64_t j = i + 1 + lane; j < n; j += 32) x[j] -= row[j] * xi;
+          else     for (int64_t j = lane; j < i; j += 32) x[j] -= row[j] * xi;
+          if (lane == 0) x[i] = xi;
+        }
+        __syncwarp();
+      }
+    }
+    for (int64_t i = lane; i < n; i += 32) b[i * nrhs] = x[i];
+    __syncwarp();  // the next pair's loads must not overtake this pair's stores of x
+  }
+}
+
+// `check` != 0 gives trtrs semantics (an exactly-zero diagonal NaN-fills B); 0 gives potrs semantics (IEEE inf / NaN
+// from the division, nothing checked) and leaves `flag` unused.
 template <typename T>
 ptk_status trsm_blocked(int dtype, const T* A, T* B, int64_t n, int64_t nrhs, int64_t ars, int64_t acs, int fwd,
-                        int unit_diag, int* flag, cudaStream_t st) {
-  PTK_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), st));
-  if (!unit_diag) diag_zero_check_kernel<T><<<(unsigned)std::min<int64_t>((n + 255) / 256, 1024), 256, 0, st>>>(A, n, ars + acs, flag);
+                        int unit_diag, int check, int* flag, cudaStream_t st) {
+  if (check) PTK_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), st));
+  if (check && !unit_diag) diag_zero_check_kernel<T><<<(unsigned)std::min<int64_t>((n + 255) / 256, 1024), 256, 0, st>>>(A, n, ars + acs, flag);
   const int64_t nblk = (n + NB - 1) / NB;
   for (int64_t b = 0; b < nblk; ++b) {
     const int64_t blk = fwd ? b : (nblk - 1 - b);
@@ -307,7 +378,7 @@ ptk_status trsm_blocked(int dtype, const T* A, T* B, int64_t n, int64_t nrhs, in
       if (s != PTK_OK) return s;
     }
   }
-  nan_fill_if_kernel<T><<<(unsigned)std::min<int64_t>((n * nrhs + 255) / 256, 2048), 256, 0, st>>>(B, n * nrhs, flag);
+  if (check) nan_fill_if_kernel<T><<<(unsigned)std::min<int64_t>((n * nrhs + 255) / 256, 2048), 256, 0, st>>>(B, n * nrhs, flag);
   PTK_LAUNCH_CHECK("trsm_blocked");
   return PTK_OK;
 }
@@ -377,10 +448,62 @@ ptk_status ptk_trsm(int dtype, const void* A, void* B, int64_t n, int64_t nrhs, 
   for (int64_t b = 0; b < batch; ++b) {
     ptk_status s = dtype == PTK_F32
                        ? trsm_blocked<float>(dtype, (const float*)A + b * n * n, (float*)B + b * n * nrhs, n, nrhs, ars, acs,
-                                             fwd, unit_diag, flag, st)
+                                             fwd, unit_diag, 1, flag, st)
                        : trsm_blocked<double>(dtype, (const double*)A + b * n * n, (double*)B + b * n * nrhs, n, nrhs, ars,
-                                              acs, fwd, unit_diag, flag, st);
+                                              acs, fwd, unit_diag, 1, flag, st);
     if (s != PTK_OK) return s;
+  }
+  return PTK_OK;
+}
+
+ptk_status ptk_potrs(int dtype, const void* C, void* B, int64_t n, int64_t nrhs, int lower, int nbatch_dims,
+                     const int64_t* batch_shape, const int64_t* factor_batch_strides, void* stream) {
+  PTK_REQUIRE_INIT();
+  if (dtype != PTK_F32 && dtype != PTK_F64) return fail(PTK_ERR_UNSUPPORTED, "ptk_potrs: dtype must be float32 or float64");
+  if (nbatch_dims < 0 || nbatch_dims > POTRS_MAX_DIMS) return fail(PTK_ERR_ARG, "ptk_potrs: at most 8 batch dimensions");
+  if (n < 0 || nrhs < 0) return fail(PTK_ERR_ARG, "ptk_potrs: negative size");
+  PotrsBatch bat{};
+  bat.nd = nbatch_dims;
+  int64_t systems = 1;
+  for (int d = 0; d < nbatch_dims; ++d) {
+    if (batch_shape[d] < 0) return fail(PTK_ERR_ARG, "ptk_potrs: negative batch dimension");
+    bat.shape[d] = batch_shape[d];
+    bat.stride[d] = factor_batch_strides[d];
+    systems *= batch_shape[d];
+  }
+  if (n == 0 || nrhs == 0 || systems == 0) return PTK_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n <= POTRS_SMALL_N) {
+    const int64_t pairs = systems * nrhs;
+    const unsigned grid = (unsigned)std::min<int64_t>((pairs + POTRS_WARPS - 1) / POTRS_WARPS,
+                                                      (int64_t)std::max(1, ptk::sm_count()) * 16);
+    if (dtype == PTK_F32)
+      potrs_small_kernel<float><<<grid, POTRS_WARPS * 32, 0, st>>>((const float*)C, (float*)B, n, nrhs, lower, bat, pairs);
+    else
+      potrs_small_kernel<double><<<grid, POTRS_WARPS * 32, 0, st>>>((const double*)C, (double*)B, n, nrhs, lower, bat, pairs);
+    PTK_LAUNCH_CHECK("potrs_small");
+    return PTK_OK;
+  }
+  // blocked path: two triangular solves per system.  lower: C y = b, then C^T x = y; upper: U^T y = b, then U x = y.
+  // op(A)(i,k) = A[i*ars + k*acs]: (n, 1) reads the stored triangle as is, (1, n) its transpose.
+  for (int64_t s = 0; s < systems; ++s) {
+    int64_t off = 0, rem = s;
+    for (int d = nbatch_dims - 1; d >= 0; --d) {
+      const int64_t q = rem / bat.shape[d];
+      off += (rem - q * bat.shape[d]) * bat.stride[d];
+      rem = q;
+    }
+    for (int sweep = 0; sweep < 2; ++sweep) {
+      const int fwd = sweep == 0 ? 1 : 0;
+      const bool plain = (sweep == 0) == (lower != 0);
+      const int64_t ars = plain ? n : 1, acs = plain ? 1 : n;
+      ptk_status r = dtype == PTK_F32
+                         ? trsm_blocked<float>(dtype, (const float*)C + off, (float*)B + s * n * nrhs, n, nrhs, ars, acs, fwd,
+                                               0, 0, nullptr, st)
+                         : trsm_blocked<double>(dtype, (const double*)C + off, (double*)B + s * n * nrhs, n, nrhs, ars, acs,
+                                                fwd, 0, 0, nullptr, st);
+      if (r != PTK_OK) return r;
+    }
   }
   return PTK_OK;
 }

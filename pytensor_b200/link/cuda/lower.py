@@ -289,6 +289,17 @@ def lower_node(node, opts):
     if cname == "SolveTriangular":
         return nlin.SolveTriangularNode(node.outputs[0].type.dtype, bool(core.lower), bool(core.unit_diagonal),
                                         int(core.b_ndim), name=str(op))
+    if cname == "CholeskySolve" or (cname == "Solve" and core.assume_a == "pos"):
+        dt = node.outputs[0].type.dtype
+        if dt not in ("float32", "float64"):
+            raise UnsupportedOp(f"{op}: output dtype {dt}")
+        nb_ = op.batch_ndim(node) if isinstance(op, Blockwise) else 0
+        bcast = tuple(tuple(i.type.broadcastable[:nb_]) for i in node.inputs)
+        if cname == "CholeskySolve":
+            return nlin.CholeskySolveNode(dt, bool(core.lower), int(core.b_ndim), bool(core.overwrite_b), bcast, name=str(op))
+        return nlin.PosSolveNode(dt, bool(core.lower), int(core.b_ndim), bcast, name=str(op))
+    if cname == "AllocDiag" and isinstance(op, Blockwise) and (core.axis1, core.axis2) == (0, 1):
+        return nlin.AllocDiagNode(core.offset, name=str(op))
 
     # more of the Op library (SURVEY.md §8(f).3)
     if cname in ("ARange", "Eye", "ExtractDiag", "Split", "Argmax", "CumOp") and not isinstance(op, Blockwise):

@@ -114,6 +114,7 @@ SIGNATURES = {
                                       c_void_p, c_void_p]),
     "ptk_potrf": (c_int, [c_int, c_void_p, c_int64, c_int64, c_int, c_void_p]),
     "ptk_trsm": (c_int, [c_int, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_int, c_int, c_void_p]),
+    "ptk_potrs": (c_int, [c_int, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, _i64p, _i64p, c_void_p]),
 }
 
 _lock = threading.Lock()
