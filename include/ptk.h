@@ -183,7 +183,8 @@ ptk_status   ptk_gemm_bias_act(int dtype, int64_t M, int64_t N, int64_t K,
  * A comes either as fp32 (A_f32, element strides sa0/sa1; staged to bf16 in the workspace) or ALREADY staged as bf16
  * (A_bf16: row-major [M,K], pitch lda_bf16 elements (multiple of 8), 16-byte aligned) — e.g. the C_bf16 copy a previous
  * call emitted, so that a chain of layers re-stages only the weights.  C_bf16 (optional, row-major pitch ldc_bf16) receives
- * a bf16 copy of the result. */
+ * a bf16 copy of the result.  Equivalent to one-piece ptk_stage_operand of A (unless A_bf16) and B^T into the workspace +
+ * ptk_gemm_tc_staged with terms 1. */
 ptk_status   ptk_gemm_tc_ex(int64_t M, int64_t N, int64_t K, double alpha, const void* A_f32, int64_t sa0, int64_t sa1,
                       const void* A_bf16, int64_t lda_bf16, const void* B_f32, int64_t sb0, int64_t sb1, double beta,
                       void* C, int64_t sc0, int64_t sc1, const void* bias, int act, void* C_bf16, int64_t ldc_bf16,
@@ -195,7 +196,9 @@ ptk_status   ptk_gemm_tc_ex(int64_t M, int64_t N, int64_t K, double alpha, const
  * wgmma kernel accumulates `terms` piece products in its fp32 register accumulator, smallest first:
  *   terms = 6: A3B1+A2B2+A1B3+A2B1+A1B2+A1B1 (only O(2^-24) products dropped: below sgemm's own rounding noise),
  *   terms = 3: A2B1+A1B2+A1B1 (about 4e-6 of the output scale at K = 4096; twice as fast).
- * workspace >= ptk_gemm_split_workspace_bytes(M, N, K), caller-owned. */
+ * workspace >= ptk_gemm_split_workspace_bytes(M, N, K), caller-owned.  Equivalent to three-piece ptk_stage_operand of A and
+ * B^T into the workspace (aligned when terms = 6 and ptk_gemm_exact_main_default()) + ptk_gemm_tc_staged with those
+ * operands' flags. */
 size_t       ptk_gemm_split_workspace_bytes(int64_t M, int64_t N, int64_t K);
 ptk_status   ptk_gemm_tc_split(int64_t M, int64_t N, int64_t K, double alpha, const void* A_f32, int64_t sa0, int64_t sa1,
                       const void* B_f32, int64_t sb0, int64_t sb1, double beta, void* C, int64_t sc0, int64_t sc1,
@@ -228,7 +231,8 @@ ptk_status   ptk_gemm_tc_split(int64_t M, int64_t N, int64_t K, double alpha, co
  *     the pieces in fp32, giving sgemm's ±inf / NaN instead of the NaN of inf * 0 piece products.  c_flags (nullable,
  *     zeroed by the caller, 3-piece C_stage only) receives the same flags for the rows of C_stage.  An epilogue-written
  *     operand carries flags only through c_flags.
- *   ptk_gemm_exact_main_default: 1 unless PTK_GEMM_EXACT=0 — what ptk_gemm_tc_split uses. */
+ *   ptk_gemm_exact_main_default: 1 unless PTK_GEMM_EXACT=0 — whether ptk_gemm_tc_split stages aligned operands and runs
+ *     ptk_gemm_tc_staged with exact_main at terms = 6. */
 #define PTK_STAGE_NO_EXP (-100000)
 size_t       ptk_stage_bytes(int64_t rows, int64_t cols, int pieces);
 ptk_status   ptk_stage_operand(const void* src_f32, int64_t sr, int64_t sc, int64_t rows, int64_t cols, int pieces, int aligned,

@@ -6,9 +6,10 @@
 #include "ptk_common.h"
 
 namespace ptk {
-ptk_status gemm_tc(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t sa0, int64_t sa1,
-                   const float* B, int64_t sb0, int64_t sb1, float beta, float* C, int64_t sc0, int64_t sc1,
-                   const float* bias, int act, void* workspace, size_t workspace_bytes, cudaStream_t st);
+ptk_status gemm_tc_ex(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t sa0, int64_t sa1,
+                      const void* A_bf16, int64_t lda_bf16, const float* B, int64_t sb0, int64_t sb1, float beta, float* C,
+                      int64_t sc0, int64_t sc1, const float* bias, int act, void* C_bf16, int64_t ldc_bf16, void* workspace,
+                      size_t workspace_bytes, cudaStream_t st);
 size_t gemm_tc_workspace(int64_t M, int64_t N, int64_t K);
 }  // namespace ptk
 
@@ -732,8 +733,8 @@ ptk_status ptk_gemm_bias_act(int dtype, int64_t M, int64_t N, int64_t K, const v
   cudaStream_t st = (cudaStream_t)stream;
   if (precision == 1) {
     if (dtype != PTK_F32) return fail(PTK_ERR_UNSUPPORTED, "ptk_gemm: the bf16 tensor-core path takes fp32 graphs only");
-    return ptk::gemm_tc(M, N, K, 1.0f, (const float*)A, sa0, sa1, (const float*)B, sb0, sb1, 0.0f, (float*)C, sc0,
-                        sc1, (const float*)bias, act, workspace, workspace_bytes, st);
+    return ptk::gemm_tc_ex(M, N, K, 1.0f, (const float*)A, sa0, sa1, nullptr, 0, (const float*)B, sb0, sb1, 0.0f, (float*)C,
+                           sc0, sc1, (const float*)bias, act, nullptr, 0, workspace, workspace_bytes, st);
   }
   if (dtype == PTK_F32) return launch_gemm<float>(M, N, K, 1.0, A, sa0, sa1, B, sb0, sb1, 0.0, C, sc0, sc1, bias, act, st);
   if (dtype == PTK_F64) return launch_gemm<double>(M, N, K, 1.0, A, sa0, sa1, B, sb0, sb1, 0.0, C, sc0, sc1, bias, act, st);
@@ -778,8 +779,8 @@ ptk_status ptk_gemm(int dtype, int64_t M, int64_t N, int64_t K, double alpha, co
   cudaStream_t st = (cudaStream_t)stream;
   if (precision == 1) {
     if (dtype != PTK_F32) return fail(PTK_ERR_UNSUPPORTED, "ptk_gemm: the bf16 tensor-core path takes fp32 graphs only");
-    return ptk::gemm_tc(M, N, K, (float)alpha, (const float*)A, sa0, sa1, (const float*)B, sb0, sb1, (float)beta,
-                        (float*)C, sc0, sc1, nullptr, 0, workspace, workspace_bytes, st);
+    return ptk::gemm_tc_ex(M, N, K, (float)alpha, (const float*)A, sa0, sa1, nullptr, 0, (const float*)B, sb0, sb1,
+                           (float)beta, (float*)C, sc0, sc1, nullptr, 0, nullptr, 0, workspace, workspace_bytes, st);
   }
   if (dtype == PTK_F32) return launch_gemm<float>(M, N, K, alpha, A, sa0, sa1, B, sb0, sb1, beta, C, sc0, sc1, nullptr, 0, st);
   if (dtype == PTK_F64) return launch_gemm<double>(M, N, K, alpha, A, sa0, sa1, B, sb0, sb1, beta, C, sc0, sc1, nullptr, 0, st);

@@ -726,48 +726,6 @@ static int exact_main_default() {
   return g;
 }
 
-// A_f32 (any strides) OR A_bf16 (row-major, pitch lda_bf16 elements, multiple of 8, 16-byte aligned base) must be given.
-ptk_status gemm_tc_ex(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t sa0, int64_t sa1,
-                      const void* A_bf16, int64_t lda_bf16, const float* B, int64_t sb0, int64_t sb1, float beta, float* C,
-                      int64_t sc0, int64_t sc1, const float* bias, int act, void* C_bf16, int64_t ldc_bf16, void* workspace,
-                      size_t workspace_bytes, cudaStream_t st) {
-  if (M == 0 || N == 0) return PTK_OK;
-  if (M > 2147483647LL || N > 2147483647LL || K > 2147483647LL) return fail(PTK_ERR_ARG, "gemm_tc: dims exceed int32");
-  if (workspace == nullptr || workspace_bytes < gemm_tc_workspace(M, N, K))
-    return fail(PTK_ERR_ARG, "gemm_tc: workspace too small (see ptk_gemm_workspace_bytes)");
-  const long long Kp = round_up(K, 8);
-  uintptr_t w = ((uintptr_t)workspace + 255) & ~(uintptr_t)255;
-  __nv_bfloat16* Abf = reinterpret_cast<__nv_bfloat16*>(w);
-  __nv_bfloat16* Bbf = reinterpret_cast<__nv_bfloat16*>(w + round_up(M * Kp * 2, 256));
-  long long lda = Kp;
-  if (A_bf16 != nullptr) {
-    if (lda_bf16 % 8 != 0 || ((uintptr_t)A_bf16 & 15) != 0) return fail(PTK_ERR_ARG, "gemm_tc: misaligned bf16 A operand");
-    Abf = reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(A_bf16));
-    lda = lda_bf16;
-  } else {
-    dim3 ga((unsigned)((K + 63) / 64), (unsigned)((M + 63) / 64));
-    convert_bf16_kernel<<<ga, 256, 0, st>>>(A, sa0, sa1, Abf, Kp, M, K);
-  }
-  {
-    // B[K,N] -> Bt[N,K]: dst row index = n (source stride sb1), dst col index = k (source stride sb0)
-    dim3 gb((unsigned)((K + 63) / 64), (unsigned)((N + 63) / 64));
-    convert_bf16_kernel<<<gb, 256, 0, st>>>(B, sb1, sb0, Bbf, Kp, N, K);
-    PTK_LAUNCH_CHECK("convert_bf16");
-  }
-  CUtensorMap ta, tb;
-  ptk_status s;
-  if ((s = make_tmap(&ta, Abf, (uint64_t)M, (uint64_t)K, (uint64_t)lda, BLOCK_M)) != PTK_OK) return s;
-  if ((s = make_tmap(&tb, Bbf, (uint64_t)N, (uint64_t)K, (uint64_t)Kp, BLOCK_N)) != PTK_OK) return s;
-  EpiParams p;
-  p.alpha = alpha; p.beta = beta; p.C = C; p.sc0 = sc0; p.sc1 = sc1; p.bias = bias; p.act = act;
-  p.M = (int)M; p.N = (int)N; p.K = (int)K;
-  p.Cbf = reinterpret_cast<__nv_bfloat16*>(C_bf16);
-  p.ldcbf = ldc_bf16;
-  p.terms = 1; p.a_rows = 0; p.b_rows = 0; p.kchunk = 0; p.out_pieces = 1; p.cbf_rows = 0; p.exact_main = 0; p.out_exp = PTK_NO_EXP; p.out_scale = 1.0f; p.out_inv = 1.0f;
-  p.fa = p.fb = nullptr; p.fc = nullptr; p.As = p.Bs = nullptr; p.lda = p.ldb = 0;   // bf16 operands: inf * 0 = NaN is the model
-  return launch_gemm(ta, tb, p, st);
-}
-
 // accumulation chunk of the fp32-accurate modes: 8 k-blocks (K = 512) keeps the tensor core's truncation bias near 1e-6 of
 // the output scale; PTK_GEMM_KCHUNK=<k-blocks> overrides (0 = one chunk)
 static int split_kchunk(int64_t K, int exact) {
@@ -817,6 +775,7 @@ ptk_status stage_operand(const float* src, int64_t sr, int64_t sc, int64_t R, in
 // pitch lda, piece pitch a_rows rows), B_stage = pieces of B^T [N,K]; terms 1 (plain bf16) | 3 | 6.  C_stage (optional)
 // receives `out_pieces` (1 | 3) staged pieces of the RESULT [M,N] (pitch ldc_stage, piece pitch c_rows) — the A operand
 // of the next product of a chain / recurrence, so that only the very first operand is ever staged by a separate pass.
+// The only code that builds the kernel's tensor maps and EpiParams: gemm_tc_ex / gemm_tc_split stage and come here.
 ptk_status gemm_tc_staged(int64_t M, int64_t N, int64_t K, float alpha, const void* A_stage, int64_t lda, int64_t a_rows,
                           const void* B_stage, int64_t ldb, int64_t b_rows, int terms, float beta, float* C, int64_t sc0,
                           int64_t sc1, const float* bias, int act, void* C_stage, int64_t ldc_stage, int64_t c_rows,
@@ -824,14 +783,22 @@ ptk_status gemm_tc_staged(int64_t M, int64_t N, int64_t K, float alpha, const vo
                           const unsigned int* b_flags, unsigned int* c_flags, cudaStream_t st) {
   if (M == 0 || N == 0) return PTK_OK;
   if (terms != 1 && terms != 3 && terms != 6) return fail(PTK_ERR_ARG, "gemm_tc_staged: terms must be 1, 3 or 6");
-  if (M > 500000000LL || N > 500000000LL || K > 2147483647LL || K <= 0) return fail(PTK_ERR_ARG, "gemm_tc_staged: bad dims");
+  // Three stacked pieces put row coordinates up to 2 * a_rows + M into the tensor map: M, N <= 5e8 keep them in int32.
+  // The one-piece product accepts what ptk_gemm_tc_ex always has: M, N up to int32 and a C_stage at any pitch (the
+  // epilogue checks the alignment of every store).
+  const bool one = terms == 1;
+  const long long max_mn = one ? 2147483647LL : 500000000LL;
+  if (M > max_mn || N > max_mn || K > 2147483647LL || K <= 0) return fail(PTK_ERR_ARG, "gemm_tc_staged: bad dims");
   if (lda % 8 || ldb % 8 || ((uintptr_t)A_stage & 15) || ((uintptr_t)B_stage & 15))
     return fail(PTK_ERR_ARG, "gemm_tc_staged: operand pitch must be a multiple of 8 elements, base 16-byte aligned");
   if (C_stage != nullptr && (out_pieces != 1 && out_pieces != 3)) return fail(PTK_ERR_ARG, "gemm_tc_staged: out_pieces must be 1 or 3");
-  if (C_stage != nullptr && (ldc_stage % 8 || ((uintptr_t)C_stage & 15))) return fail(PTK_ERR_ARG, "gemm_tc_staged: misaligned C_stage");
-  const int pa = terms == 1 ? 1 : 3;
+  if (C_stage != nullptr && !one && (ldc_stage % 8 || ((uintptr_t)C_stage & 15)))
+    return fail(PTK_ERR_ARG, "gemm_tc_staged: misaligned C_stage");
+  const int pa = one ? 1 : 3;
   CUtensorMap ta, tb;
   ptk_status s;
+  // rows past M (N) inside a piece hold whatever the staging buffer held: they only reach output rows (columns) the
+  // epilogue masks, never a stored element; columns past K and rows past the last piece are zero-filled by TMA
   const uint64_t a_total = (uint64_t)((pa - 1) * a_rows + M), b_total = (uint64_t)((pa - 1) * b_rows + N);
   if ((s = make_tmap(&ta, A_stage, a_total, (uint64_t)K, (uint64_t)lda, BLOCK_M)) != PTK_OK) return s;
   if ((s = make_tmap(&tb, B_stage, b_total, (uint64_t)K, (uint64_t)ldb, BLOCK_N)) != PTK_OK) return s;
@@ -842,26 +809,51 @@ ptk_status gemm_tc_staged(int64_t M, int64_t N, int64_t K, float alpha, const vo
   p.ldcbf = ldc_stage;
   p.out_pieces = C_stage ? out_pieces : 1;
   p.cbf_rows = c_rows;
-  p.exact_main = 0; p.out_exp = PTK_NO_EXP; p.out_scale = 1.0f; p.out_inv = 1.0f;
-  p.terms = terms; p.a_rows = terms == 1 ? 0 : (int)a_rows; p.b_rows = terms == 1 ? 0 : (int)b_rows;
-  p.exact_main = (terms != 1 && exact_main) ? 1 : 0;
+  p.terms = terms; p.a_rows = one ? 0 : (int)a_rows; p.b_rows = one ? 0 : (int)b_rows;
+  p.exact_main = (!one && exact_main) ? 1 : 0;
   p.out_exp = (C_stage && out_pieces == 3) ? out_exp : PTK_NO_EXP;
+  p.out_scale = 1.0f; p.out_inv = 1.0f;
   if (p.out_exp != PTK_NO_EXP) {
     if (p.out_exp < -100 || p.out_exp > 100) return fail(PTK_ERR_ARG, "gemm_tc_staged: out_exp out of range");
     p.out_scale = ldexpf(1.0f, p.out_exp);
     p.out_inv = ldexpf(1.0f, -p.out_exp);
   }
-  p.kchunk = terms == 1 ? 0 : split_kchunk(K, p.exact_main);
-  const bool three = terms != 1;   // (flags only mean something for three-piece operands / outputs)
-  p.fa = three ? a_flags : nullptr; p.fb = three ? b_flags : nullptr;
+  p.kchunk = one ? 0 : split_kchunk(K, p.exact_main);
+  p.fa = one ? nullptr : a_flags; p.fb = one ? nullptr : b_flags;   // (flags only mean something for three-piece operands)
   p.fc = (C_stage && out_pieces == 3) ? c_flags : nullptr;
   p.As = reinterpret_cast<const __nv_bfloat16*>(A_stage); p.Bs = reinterpret_cast<const __nv_bfloat16*>(B_stage);
   p.lda = lda; p.ldb = ldb;
   return launch_gemm(ta, tb, p, st);
 }
 
-// fp32-accurate product on the tensor cores: both operands split into three bf16 pieces, `terms` (3 or 6) piece products
-// per k-block accumulated in fp32 registers by the wgmma kernel (see EpiParams::terms).
+// bf16 product with fp32 operands: A (unless given as A_bf16: row-major, pitch lda_bf16 elements, multiple of 8, 16-byte
+// aligned base) and B^T are staged as one bf16 piece each in the workspace, then multiplied by gemm_tc_staged.
+ptk_status gemm_tc_ex(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t sa0, int64_t sa1,
+                      const void* A_bf16, int64_t lda_bf16, const float* B, int64_t sb0, int64_t sb1, float beta, float* C,
+                      int64_t sc0, int64_t sc1, const float* bias, int act, void* C_bf16, int64_t ldc_bf16, void* workspace,
+                      size_t workspace_bytes, cudaStream_t st) {
+  if (M == 0 || N == 0) return PTK_OK;
+  if (M > 2147483647LL || N > 2147483647LL || K > 2147483647LL) return fail(PTK_ERR_ARG, "gemm_tc: dims exceed int32");
+  if (workspace == nullptr || workspace_bytes < gemm_tc_workspace(M, N, K))
+    return fail(PTK_ERR_ARG, "gemm_tc: workspace too small (see ptk_gemm_workspace_bytes)");
+  const long long Kp = round_up(K, 8);
+  uintptr_t w = ((uintptr_t)workspace + 255) & ~(uintptr_t)255;
+  void* Bbf = reinterpret_cast<void*>(w + round_up(M * Kp * 2, 256));
+  ptk_status s;
+  if (A_bf16 == nullptr) {
+    void* Abf = reinterpret_cast<void*>(w);
+    if ((s = stage_operand(A, sa0, sa1, M, K, 1, Abf, Kp, 0, 0, nullptr, st)) != PTK_OK) return s;
+    A_bf16 = Abf;
+    lda_bf16 = Kp;
+  }
+  if ((s = stage_operand(B, sb1, sb0, N, K, 1, Bbf, Kp, 0, 0, nullptr, st)) != PTK_OK) return s;   // B[K,N] -> Bt[N,K]
+  return gemm_tc_staged(M, N, K, alpha, A_bf16, lda_bf16, 0, Bbf, Kp, 0, 1, beta, C, sc0, sc1, bias, act, C_bf16, ldc_bf16, 0,
+                        1, 0, PTK_NO_EXP, nullptr, nullptr, nullptr, st);
+}
+
+// fp32-accurate product on the tensor cores: both operands split into three bf16 pieces in the workspace (the per-row
+// words behind them: sexp for A, sexp + M for B^T), then `terms` (3 or 6) piece products per k-block by gemm_tc_staged
+// (see EpiParams::terms).
 ptk_status gemm_tc_split(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t sa0, int64_t sa1, const float* B,
                          int64_t sb0, int64_t sb1, float beta, float* C, int64_t sc0, int64_t sc1, const float* bias, int act,
                          int terms, void* workspace, size_t workspace_bytes, cudaStream_t st) {
@@ -872,40 +864,16 @@ ptk_status gemm_tc_split(int64_t M, int64_t N, int64_t K, float alpha, const flo
     return fail(PTK_ERR_ARG, "gemm_tc_split: workspace too small (see ptk_gemm_split_workspace_bytes)");
   const long long Kp = round_up(K, 8), Mp = round_up(M, 256), Np = round_up(N, 256);
   uintptr_t w = ((uintptr_t)workspace + 255) & ~(uintptr_t)255;
-  __nv_bfloat16* Abf = reinterpret_cast<__nv_bfloat16*>(w);
-  __nv_bfloat16* Bbf = reinterpret_cast<__nv_bfloat16*>(w + round_up(3 * Mp * Kp * 2, 256));
-  const int exact = terms == 6 ? exact_main_default() : 0;   // (3 terms need the 8-bit leading pieces of the plain split)
+  void* Abf = reinterpret_cast<void*>(w);
+  void* Bbf = reinterpret_cast<void*>(w + round_up(3 * Mp * Kp * 2, 256));
   int* sexp = reinterpret_cast<int*>(w + round_up(3 * Mp * Kp * 2, 256) + round_up(3 * Np * Kp * 2, 256));
-  {
-    ptk_status ss;
-    if ((ss = stage_operand(A, sa0, sa1, M, K, 3, Abf, Kp, Mp, exact, sexp, st)) != PTK_OK) return ss;
-    if ((ss = stage_operand(B, sb1, sb0, N, K, 3, Bbf, Kp, Np, exact, sexp + M, st)) != PTK_OK) return ss;  // B[K,N] -> Bt[N,K]
-  }
-  CUtensorMap ta, tb;
+  const int exact = terms == 6 ? exact_main_default() : 0;   // (3 terms need the 8-bit leading pieces of the plain split)
   ptk_status s;
-  // rows past M (N) inside a piece hold whatever the workspace held: they only reach output rows (columns) the epilogue
-  // masks, never a stored element; columns past K are zero-filled by TMA (the map's extent is K)
-  if ((s = make_tmap(&ta, Abf, (uint64_t)(3 * Mp), (uint64_t)K, (uint64_t)Kp, BLOCK_M)) != PTK_OK) return s;
-  if ((s = make_tmap(&tb, Bbf, (uint64_t)(3 * Np), (uint64_t)K, (uint64_t)Kp, BLOCK_N)) != PTK_OK) return s;
-  EpiParams p;
-  p.alpha = alpha; p.beta = beta; p.C = C; p.sc0 = sc0; p.sc1 = sc1; p.bias = bias; p.act = act;
-  p.M = (int)M; p.N = (int)N; p.K = (int)K;
-  p.Cbf = nullptr;
-  p.ldcbf = 0;
-  p.out_pieces = 1; p.cbf_rows = 0; p.exact_main = 0; p.out_exp = PTK_NO_EXP; p.out_scale = 1.0f; p.out_inv = 1.0f;
-  p.terms = terms; p.a_rows = (int)Mp; p.b_rows = (int)Np;
-  p.exact_main = exact;
-  p.kchunk = split_kchunk(K, exact);
-  p.fa = reinterpret_cast<const unsigned int*>(sexp); p.fb = reinterpret_cast<const unsigned int*>(sexp + M); p.fc = nullptr;
-  p.As = Abf; p.Bs = Bbf; p.lda = Kp; p.ldb = Kp;
-  return launch_gemm(ta, tb, p, st);
-}
-
-ptk_status gemm_tc(int64_t M, int64_t N, int64_t K, float alpha, const float* A, int64_t sa0, int64_t sa1,
-                   const float* B, int64_t sb0, int64_t sb1, float beta, float* C, int64_t sc0, int64_t sc1,
-                   const float* bias, int act, void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  return gemm_tc_ex(M, N, K, alpha, A, sa0, sa1, nullptr, 0, B, sb0, sb1, beta, C, sc0, sc1, bias, act, nullptr, 0, workspace,
-                    workspace_bytes, st);
+  if ((s = stage_operand(A, sa0, sa1, M, K, 3, Abf, Kp, Mp, exact, sexp, st)) != PTK_OK) return s;
+  if ((s = stage_operand(B, sb1, sb0, N, K, 3, Bbf, Kp, Np, exact, sexp + M, st)) != PTK_OK) return s;   // B[K,N] -> Bt[N,K]
+  const unsigned int* flags = reinterpret_cast<const unsigned int*>(sexp);
+  return gemm_tc_staged(M, N, K, alpha, Abf, Kp, Mp, Bbf, Kp, Np, terms, beta, C, sc0, sc1, bias, act, nullptr, 0, 0, 1, exact,
+                        PTK_NO_EXP, flags, flags + M, nullptr, st);
 }
 
 }  // namespace ptk

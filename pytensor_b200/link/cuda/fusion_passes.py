@@ -77,8 +77,8 @@ def fuse_gemm_epilogue(steps, output_slots, opts):
 
 
 def mark_bf16_chains(steps):
-    """A tensor-core GEMM whose result is the A operand of another tensor-core GEMM also emits a bf16 copy of it
-    (carried as `Val.aux`), so the chain re-stages only the weights (SURVEY.md §8d cfg 3)."""
+    """A tensor-core GEMM whose result is the A operand of another tensor-core GEMM also emits it staged as that operand
+    (a nodes_blas.Staged carried as `Val.aux`), so the chain re-stages only the weights (SURVEY.md §8d cfg 3)."""
     tc = (Dot22Node, GemmBiasActNode)
     producers = {o: st for st in steps for o in st.outs}
     for st in steps:

@@ -132,8 +132,6 @@ class _TraceLib:
     def __getattr__(self, name):
         if name == "ptk_sm_count":
             return lambda: 132  # H100 SXM
-        if name == "ptk_gemm_workspace_bytes":
-            return lambda M, N, K, p: 2 * (M * K + N * K) + 1024
         if name == "ptk_put_rows_workspace_bytes":
             return lambda n_dst, n_idx: 4 * (n_dst + 1 + n_idx) + 64
         if name == "ptk_stage_bytes":
@@ -142,8 +140,6 @@ class _TraceLib:
             return lambda: 1
         if name == "ptk_gemm_lead_bits":
             return lambda K: 7
-        if name == "ptk_gemm_split_workspace_bytes":
-            return lambda M, N, K: 6 * ((M + 255) // 256 * 256 + (N + 255) // 256 * 256) * ((K + 7) // 8 * 8) + 4 * (M + N) + 1024
         if name == "ptk_nonzero_workspace_bytes":
             return lambda n: 8 * ((n + 4095) // 4096 + 1)
         if name == "ptk_last_error":

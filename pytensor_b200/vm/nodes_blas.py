@@ -1,6 +1,7 @@
 """BLAS-family nodes (reference: pytensor/tensor/blas/gemm.py:76 Gemm, :248 Dot22, :298 Dot22Scalar,
 gemv.py:16 Gemv, ger.py:8 Ger, and the generic Dot of pytensor/tensor/math.py).  All arithmetic runs in
-ptk_gemm / ptk_gemv / ptk_ger; `precision` selects the bf16 wgmma tensor-core path for fp32 matrices."""
+ptk_gemm / ptk_gemv / ptk_ger, and for large fp32 matrices in the wgmma tensor-core kernel: operands staged by
+ptk_stage_operand, the product by ptk_gemm_tc_staged; `precision` 1 selects bf16 operands there."""
 
 from __future__ import annotations
 
@@ -15,96 +16,57 @@ from .values import Val
 
 # Linker-level knob: 0 = fp32-accurate (<= 1e-5 vs BLAS); 1 = bf16 operands / fp32 accumulation
 TC_MIN_DIM = 256
-# How precision 0 multiplies large fp32 matrices: "tc6" / "tc3" = wgmma with every operand split into three bf16 pieces
-# and 6 / 3 piece products per k-block (include/ptk.h ptk_gemm_tc_split; 6 terms is more accurate than sgemm itself,
-# 3 terms ~4e-6 of the output scale), "simt" = the fp32 FMA kernel.  fp64 and small / skinny products always take FMA.
+# How precision 0 multiplies large fp32 matrices: "tc6" / "tc3" = wgmma with every operand staged as three bf16 pieces
+# and 6 / 3 piece products per k-block (include/ptk.h ptk_stage_operand + ptk_gemm_tc_staged; 6 terms is more accurate
+# than sgemm itself, 3 terms ~4e-6 of the output scale), "simt" = the fp32 FMA kernel.  fp64 and small / skinny products
+# always take FMA.
 import os as _os
 
 FP32_MODE = _os.environ.get("PTK_GEMM_FP32", "tc6")
-
-_workspace = {"buf": None}
-
-
-def _get_workspace(nbytes: int):
-    buf = _workspace["buf"]
-    if buf is None or buf.numel() < nbytes:
-        buf = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=dev.device())
-        _workspace["buf"] = buf
-    return buf
 
 
 def _scalar(v: Val) -> float:
     return float(np.asarray(v.host()).reshape(-1)[0])
 
 
-def gemm(dtype, alpha, A, B, beta, C, precision=0, bias=None, act=0, a_bf16=None, want_bf16=False, b_key=None):
+def _zero_fill(t: torch.Tensor) -> None:
+    """t = 0 for a dense buffer: the result of a product whose contraction is empty."""
+    _lib.check(_lib.lib().ptk_memset_async(dev.ptr(t), 0, t.numel() * t.element_size(), dev.stream_ptr()), "memset")
+
+
+def gemm(dtype, alpha, A, B, beta, C, precision=0, bias=None, act=0, a_staged=None, want_staged=False, b_key=None):
     """C = alpha*A@B + beta*C (or act(A@B + bias) when bias/act given) through the C-ABI.
-    Tensor-core path extras: `a_bf16` = an already staged bf16 copy of A (skips the staging pass); `want_bf16` returns a
-    bf16 copy of C (torch.bfloat16 container) for the next layer, else None."""
+    Tensor-core path extras: `a_staged` = A as the previous product's epilogue staged it (used instead of staging A when
+    it fits this product); `want_staged` returns the result staged as the A operand of the next product, else None."""
     M, K = A.shape
     K2, N = B.shape
     if K != K2 or tuple(C.shape) != (M, N):
         raise ValueError(f"gemm: shape mismatch {tuple(A.shape)} @ {tuple(B.shape)} -> {tuple(C.shape)}")
+    plan = tc_plan(dtype, precision, M, N, K)
+    if plan is not None:
+        pieces, terms = plan
+        # B: the resident staged copy when the VM knows its content, else staged per call
+        Bst = staged_weight(b_key, B, pieces)
+        resident = Bst is not None
+        if not resident:
+            Bst = stage_operand(B, pieces, transposed=True)
+        # Three-piece operands chain only between products with a resident B.  An epilogue splits its result on the
+        # fixed 2^-6 grid of a tanh output, staging splits on a per-row grid: a chained A changes the product's bits,
+        # so a product whose weights are staged per call computes from A staged by itself, as it always has.
+        chain = pieces == 1 or resident
+        if chain and isinstance(a_staged, Staged) and \
+                (a_staged.pieces, a_staged.rows, a_staged.cols, a_staged.aligned) == (pieces, M, K, Bst.aligned):
+            Ast = a_staged
+        else:
+            Ast = stage_operand(A, pieces, aligned=Bst.aligned)
+        out = None
+        if want_staged and chain and (pieces == 1 or can_chain_pieces(act)):
+            out = Staged(M, N, pieces, aligned=Bst.aligned)
+        gemm_staged(Ast, Bst, terms, alpha, beta, C, bias=bias, act=act, out=out)
+        return out
     L = _lib.lib()
-    use_tc = precision == 1 and dtype == "float32" and min(M, N, K) >= TC_MIN_DIM
     code = _lib.DTYPE_CODE[dtype]
     st = dev.stream_ptr()
-    plan = tc_plan(dtype, precision, M, N, K) if b_key is not None else None
-    if plan is not None:
-        # resident weights: B comes from the staged-operand cache, only A is staged per call (or chained from the
-        # previous layer's epilogue in the bf16 mode)
-        pieces, terms = plan
-        Bst = staged_weight(b_key, B, pieces)
-        if Bst is not None:
-            if isinstance(a_bf16, Staged):
-                ok = (a_bf16.pieces, a_bf16.rows, a_bf16.cols, a_bf16.aligned) == (pieces, M, K, Bst.aligned)
-                Ast = a_bf16 if ok else stage_operand(A, pieces, aligned=Bst.aligned)
-            elif pieces == 1 and a_bf16 is not None and a_bf16.shape[0] == M and a_bf16.shape[1] >= K \
-                    and a_bf16.stride(1) == 1 and a_bf16.stride(0) % 8 == 0 and dev.ptr(a_bf16) % 16 == 0:
-                Ast = Staged.wrap(a_bf16, M, K)
-            else:
-                Ast = stage_operand(A, pieces, aligned=Bst.aligned)
-            ret = cst = None
-            if want_bf16 and pieces == 1:
-                ret = dev.empty_t((M, (N + 7) // 8 * 8), torch.bfloat16)
-                cst = Staged.wrap(ret, M, N)
-            elif want_bf16 and can_chain_pieces(act):
-                ret = cst = Staged(M, N, pieces, aligned=Bst.aligned)   # the three-piece operand of the next product
-            gemm_staged(Ast, Bst, terms, alpha, beta, C, bias=bias, act=act, out=cst)
-            return ret
-    if isinstance(a_bf16, Staged):
-        a_bf16 = None   # (a chained three-piece operand is only usable together with a resident B)
-    if use_tc:
-        ws_bytes = int(L.ptk_gemm_workspace_bytes(M, N, K, 1))
-        if dev.alloc_state.arena is not None or dev.alloc_state.measuring:
-            # inside a captured graph GEMMs may run concurrently on different streams: each gets its own staging area
-            ws = dev.empty_t((ws_bytes,), torch.uint8)
-        else:
-            ws = _get_workspace(ws_bytes)
-        cbf = None
-        if want_bf16:
-            Np = (N + 7) // 8 * 8
-            cbf = dev.empty_t((M, Np), torch.bfloat16)
-        abf_ptr, lda = None, 0
-        if a_bf16 is not None and a_bf16.shape[0] == M and a_bf16.shape[1] >= K and a_bf16.stride(1) == 1:
-            abf_ptr, lda = dev.ptr(a_bf16), a_bf16.stride(0)
-        _lib.check(L.ptk_gemm_tc_ex(M, N, K, float(alpha), dev.ptr(A), A.stride(0), A.stride(1), abf_ptr, lda, dev.ptr(B),
-                                    B.stride(0), B.stride(1), float(beta), dev.ptr(C), C.stride(0), C.stride(1),
-                                    dev.ptr(bias) if bias is not None else None, act,
-                                    dev.ptr(cbf) if cbf is not None else None, cbf.stride(0) if cbf is not None else 0,
-                                    dev.ptr(ws), ws_bytes, st), "ptk_gemm_tc_ex")
-        return cbf
-    if precision == 0 and dtype == "float32" and FP32_MODE in ("tc6", "tc3") and min(M, N, K) >= TC_MIN_DIM:
-        ws_bytes = int(L.ptk_gemm_split_workspace_bytes(M, N, K))
-        if dev.alloc_state.arena is not None or dev.alloc_state.measuring:
-            ws = dev.empty_t((ws_bytes,), torch.uint8)
-        else:
-            ws = _get_workspace(ws_bytes)
-        _lib.check(L.ptk_gemm_tc_split(M, N, K, float(alpha), dev.ptr(A), A.stride(0), A.stride(1), dev.ptr(B), B.stride(0),
-                                       B.stride(1), float(beta), dev.ptr(C), C.stride(0), C.stride(1),
-                                       dev.ptr(bias) if bias is not None else None, act, 6 if FP32_MODE == "tc6" else 3,
-                                       dev.ptr(ws), ws_bytes, st), "ptk_gemm_tc_split")
-        return None
     if bias is not None or act:
         _lib.check(L.ptk_gemm_bias_act(code, M, N, K, dev.ptr(A), A.stride(0), A.stride(1), dev.ptr(B), B.stride(0),
                                        B.stride(1), dev.ptr(bias) if bias is not None else None, act, dev.ptr(C),
@@ -132,14 +94,6 @@ class Staged:
 
     __slots__ = ("buf", "rows", "cols", "ld", "piece_rows", "pieces", "in_graph", "aligned", "flagged")
 
-    @classmethod
-    def wrap(cls, t: torch.Tensor, rows, cols):
-        """A caller-provided row-major bf16 matrix (pitch multiple of 8, 16-byte aligned) as a one-piece operand."""
-        st = cls.__new__(cls)
-        st.rows, st.cols, st.pieces, st.ld, st.piece_rows, st.buf, st.in_graph = int(rows), int(cols), 1, int(t.stride(0)), 0, t, False
-        st.aligned = st.flagged = False
-        return st
-
     def __init__(self, rows, cols, pieces, aligned=False):
         self.in_graph = False
         self.flagged = False   # the ±inf row flags behind the pieces are valid (see flags_ptr)
@@ -152,8 +106,6 @@ class Staged:
 
     @property
     def ptr(self):
-        if self.buf.dtype != torch.uint8:   # a caller-provided bf16 matrix used as is (already 16-byte aligned)
-            return dev.ptr(self.buf)
         return (dev.ptr(self.buf) + 255) & ~255
 
     @property
@@ -293,11 +245,10 @@ class Dot22Node(Node):
         aux = None
         if out.numel():
             if A.shape[1] == 0:
-                _lib.check(_lib.lib().ptk_memset_async(dev.ptr(out), 0, out.numel() * out.element_size(),
-                                                       dev.stream_ptr()), "memset")
+                _zero_fill(out)
             else:
-                aux = gemm(self.dtype, alpha, A, B, 0.0, out, self.precision, a_bf16=vals[0].aux,
-                           want_bf16=self.emit_bf16, b_key=vals[1].key)
+                aux = gemm(self.dtype, alpha, A, B, 0.0, out, self.precision, a_staged=vals[0].aux,
+                           want_staged=self.emit_bf16, b_key=vals[1].key)
         return [Val(d=out, aux=aux)]
 
 
@@ -323,8 +274,7 @@ class GemmNode(Node):
         if out.numel():
             if X.shape[1] == 0:
                 if beta == 0.0:
-                    _lib.check(_lib.lib().ptk_memset_async(dev.ptr(out), 0, out.numel() * out.element_size(),
-                                                           dev.stream_ptr()), "memset")
+                    _zero_fill(out)
                 else:
                     gemm(self.dtype, 0.0, out[:, :1], out[:1, :], beta, out, 0)
             else:
@@ -350,8 +300,7 @@ class GemvNode(Node):
                 Am = out.as_strided((out.shape[0], 1), (out.stride(0), 1), out.storage_offset())
                 X = out[:1]
                 if be == 0.0:
-                    _lib.check(_lib.lib().ptk_memset_async(dev.ptr(out), 0, out.numel() * out.element_size(),
-                                                           dev.stream_ptr()), "memset")
+                    _zero_fill(out)
                     return [Val(d=out)]
             gemv(self.dtype, al, Am, X, be, out)
         return [Val(d=out)]
@@ -389,7 +338,7 @@ class DotNode(Node):
             out = dev.empty((A.shape[0],), self.dtype)
             if out.numel():
                 if A.shape[1] == 0:
-                    _lib.check(_lib.lib().ptk_memset_async(dev.ptr(out), 0, out.numel() * out.element_size(), dev.stream_ptr()), "memset")
+                    _zero_fill(out)
                 else:
                     gemv(self.dtype, 1.0, A, B, 0.0, out)
             return [Val(d=out)]
@@ -397,14 +346,14 @@ class DotNode(Node):
             out = dev.empty((B.shape[1],), self.dtype)
             if out.numel():
                 if B.shape[0] == 0:
-                    _lib.check(_lib.lib().ptk_memset_async(dev.ptr(out), 0, out.numel() * out.element_size(), dev.stream_ptr()), "memset")
+                    _zero_fill(out)
                 else:
                     gemv(self.dtype, 1.0, B.t(), A, 0.0, out)
             return [Val(d=out)]
         if A.dim() == 1 and B.dim() == 1:
             out = dev.empty((1,), self.dtype)
             if A.shape[0] == 0:
-                _lib.check(_lib.lib().ptk_memset_async(dev.ptr(out), 0, out.element_size(), dev.stream_ptr()), "memset")
+                _zero_fill(out)
             else:
                 Am = A.as_strided((1, A.shape[0]), (A.shape[0] * max(1, A.stride(0)), A.stride(0)), A.storage_offset())
                 gemv(self.dtype, 1.0, Am, B, 0.0, out)
@@ -435,8 +384,8 @@ class GemmBiasActNode(Node):
         if out.numel():
             if A.shape[1] == 0:
                 raise NotImplementedError("fused bias epilogue with K == 0")
-            aux = gemm(self.dtype, 1.0, A, B, 0.0, out, self.precision, bias=b1, act=self.act, a_bf16=vals[0].aux,
-                       want_bf16=self.emit_bf16, b_key=vals[1].key)
+            aux = gemm(self.dtype, 1.0, A, B, 0.0, out, self.precision, bias=b1, act=self.act, a_staged=vals[0].aux,
+                       want_staged=self.emit_bf16, b_key=vals[1].key)
             return [Val(d=out, aux=aux)]
         return [Val(d=out)]
 
@@ -457,8 +406,7 @@ class BatchedDotNode(Node):
         out = dev.empty((nb, M, N), self.dtype)
         if out.numel():
             if K == 0:
-                _lib.check(_lib.lib().ptk_memset_async(dev.ptr(out), 0, out.numel() * out.element_size(),
-                                                       dev.stream_ptr()), "memset")
+                _zero_fill(out)
             else:
                 for i in range(nb):
                     gemm(self.dtype, 1.0, A[i], B[i], 0.0, out[i], self.precision)

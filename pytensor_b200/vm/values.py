@@ -16,16 +16,20 @@ from ..runtime import device as dev
 
 
 class Val:
-    __slots__ = ("h", "d", "aux", "key")
+    __slots__ = ("h", "d", "aux", "key", "fresh")
 
-    def __init__(self, h=None, d=None, aux=None, key=None):
+    def __init__(self, h=None, d=None, aux=None, key=None, fresh=False):
         self.h = h
         self.d = d
-        self.aux = aux  # optional device-side companion of `d` (e.g. the bf16 copy a tensor-core GEMM emitted)
+        # optional companion of `d`: the same matrix staged as the A operand of the next tensor-core product
+        # (a nodes_blas.Staged written by the epilogue of the product that computed `d`), or None
+        self.aux = aux
         # identity of the CONTENT when the VM knows it cannot have changed since it last saw this key (a graph constant;
         # a caller-owned device tensor that is the same object at the same torch version as in the previous calls):
         # lets a tensor-core GEMM reuse the staged copy of a weight matrix instead of re-staging it (nodes_blas.py)
         self.key = key
+        # `h` was filled for this call alone (the chunked host pipeline's page-locked results): handed out without a copy
+        self.fresh = fresh
 
     # ---- metadata without forcing a transfer ----
     @property

@@ -543,7 +543,7 @@ class Executor:
         _lib.check(L.ptk_sync_stream(sp2), "sync")
         plan.pop("keep", None)
         self.chunked_calls += 1
-        return [Val(h=h, aux="fresh") for h in host_out]
+        return [Val(h=h, fresh=True) for h in host_out]
 
     def _capture(self, e, inputs):
         import torch
@@ -717,8 +717,8 @@ def outputs_to_host(out_vals, device_outputs=False, copy_device=False, sink=None
             res.append(v.h)   # the advanced generator of a RandomVariable node goes back as the object it is
         elif v.h is not None and v.d is None:
             # host-only values (shape vectors ...) are cached inside the VM: hand out a fresh object per call.  The
-            # chunked host pipeline's results (aux == "fresh": page-locked arrays it filled for THIS call) already are.
-            res.append(np.asarray(v.h) if isinstance(v.aux, str) and v.aux == "fresh" else np.array(v.h, copy=True))
+            # chunked host pipeline's results (Val.fresh: page-locked arrays it filled for THIS call) already are.
+            res.append(np.asarray(v.h) if v.fresh else np.array(v.h, copy=True))
         elif device_outputs:
             res.append(dev.clone(v.d) if copy_device else v.d)
         else:
