@@ -29,7 +29,8 @@ __device__ __forceinline__ float act_apply<float>(float v, int act) {
 }
 
 // C = alpha * A @ B + beta * C (+ bias[n], act). A_KFAST: A's K stride is 1; B_NFAST: B's N stride is 1 — only the
-// thread->element mapping of the global loads changes so that a warp always walks the unit-stride direction.
+// thread->element mapping of the global loads changes so that a warp always walks the unit-stride direction.  The m-tiles
+// are walked grid-stride along y (gridDim.y is capped at 65535, so products with more than 65535 * 64 rows loop).
 template <typename T, bool A_KFAST, bool B_NFAST>
 __global__ void __launch_bounds__(256) gemm_simt_kernel(int64_t M, int64_t N, int64_t K, T alpha,
                                                         const T* __restrict__ A, int64_t sa0, int64_t sa1,
@@ -40,58 +41,60 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(int64_t M, int64_t N, in
   __shared__ T Bs[BK][BN + 4];
   const int t = threadIdx.x;
   const int tx = t % 16, ty = t / 16;
-  const int64_t m0 = (int64_t)blockIdx.y * BM, n0 = (int64_t)blockIdx.x * BN;
-  T acc[TM][TN];
+  const int64_t n0 = (int64_t)blockIdx.x * BN;
+  for (int64_t m0 = (int64_t)blockIdx.y * BM; m0 < M; m0 += (int64_t)gridDim.y * BM) {  // uniform per block
+    T acc[TM][TN];
 #pragma unroll
-  for (int i = 0; i < TM; ++i)
+    for (int i = 0; i < TM; ++i)
 #pragma unroll
-    for (int j = 0; j < TN; ++j) acc[i][j] = T(0);
+      for (int j = 0; j < TN; ++j) acc[i][j] = T(0);
 
-  for (int64_t k0 = 0; k0 < K; k0 += BK) {
+    for (int64_t k0 = 0; k0 < K; k0 += BK) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      int m, k;
-      if (A_KFAST) { k = t % BK; m = t / BK + 16 * i; }
-      else         { m = t % BM; k = t / BM + 4 * i; }
-      int64_t gm = m0 + m, gk = k0 + k;
-      As[k][m] = (gm < M && gk < K) ? A[gm * sa0 + gk * sa1] : T(0);
+      for (int i = 0; i < 4; ++i) {
+        int m, k;
+        if (A_KFAST) { k = t % BK; m = t / BK + 16 * i; }
+        else         { m = t % BM; k = t / BM + 4 * i; }
+        int64_t gm = m0 + m, gk = k0 + k;
+        As[k][m] = (gm < M && gk < K) ? A[gm * sa0 + gk * sa1] : T(0);
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        int n, k;
+        if (B_NFAST) { n = t % BN; k = t / BN + 4 * i; }
+        else         { k = t % BK; n = t / BK + 16 * i; }
+        int64_t gn = n0 + n, gk = k0 + k;
+        Bs[k][n] = (gn < N && gk < K) ? B[gk * sb0 + gn * sb1] : T(0);
+      }
+      __syncthreads();
+#pragma unroll
+      for (int k = 0; k < BK; ++k) {
+        T a[TM], b[TN];
+#pragma unroll
+        for (int i = 0; i < TM; ++i) a[i] = As[k][ty * TM + i];
+#pragma unroll
+        for (int j = 0; j < TN; ++j) b[j] = Bs[k][tx * TN + j];
+#pragma unroll
+        for (int i = 0; i < TM; ++i)
+#pragma unroll
+          for (int j = 0; j < TN; ++j) acc[i][j] += a[i] * b[j];
+      }
+      __syncthreads();
     }
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      int n, k;
-      if (B_NFAST) { n = t % BN; k = t / BN + 4 * i; }
-      else         { k = t % BK; n = t / BK + 16 * i; }
-      int64_t gn = n0 + n, gk = k0 + k;
-      Bs[k][n] = (gn < N && gk < K) ? B[gk * sb0 + gn * sb1] : T(0);
-    }
-    __syncthreads();
+    for (int i = 0; i < TM; ++i) {
+      int64_t gm = m0 + ty * TM + i;
+      if (gm >= M) continue;
 #pragma unroll
-    for (int k = 0; k < BK; ++k) {
-      T a[TM], b[TN];
-#pragma unroll
-      for (int i = 0; i < TM; ++i) a[i] = As[k][ty * TM + i];
-#pragma unroll
-      for (int j = 0; j < TN; ++j) b[j] = Bs[k][tx * TN + j];
-#pragma unroll
-      for (int i = 0; i < TM; ++i)
-#pragma unroll
-        for (int j = 0; j < TN; ++j) acc[i][j] += a[i] * b[j];
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < TM; ++i) {
-    int64_t gm = m0 + ty * TM + i;
-    if (gm >= M) continue;
-#pragma unroll
-    for (int j = 0; j < TN; ++j) {
-      int64_t gn = n0 + tx * TN + j;
-      if (gn >= N) continue;
-      T* p = C + gm * sc0 + gn * sc1;
-      T v = alpha * acc[i][j];
-      if (beta != T(0)) v += beta * (*p);  // beta == 0 must not read C (it may hold NaNs from AllocEmpty)
-      if (bias) v += bias[gn];
-      *p = act_apply<T>(v, act);
+      for (int j = 0; j < TN; ++j) {
+        int64_t gn = n0 + tx * TN + j;
+        if (gn >= N) continue;
+        T* p = C + gm * sc0 + gn * sc1;
+        T v = alpha * acc[i][j];
+        if (beta != T(0)) v += beta * (*p);  // beta == 0 must not read C (it may hold NaNs from AllocEmpty)
+        if (bias) v += bias[gn];
+        *p = act_apply<T>(v, act);
+      }
     }
   }
 }
@@ -493,8 +496,7 @@ ptk_status launch_gemm(int64_t M, int64_t N, int64_t K, double alpha, const void
     PTK_LAUNCH_CHECK("gemm_smalln");
     return PTK_OK;
   }
-  dim3 grid((unsigned)((N + BN - 1) / BN), (unsigned)((M + BM - 1) / BM));
-  if (grid.y > 65535) return ptk::fail(PTK_ERR_UNSUPPORTED, "ptk_gemm: M too large for the SIMT path");
+  dim3 grid((unsigned)((N + BN - 1) / BN), (unsigned)std::min<int64_t>((M + BM - 1) / BM, 65535));
   bool akf = (sa1 == 1) || K == 1, bnf = (sb1 == 1) || N == 1;
   if (sa0 == 1 && sa1 != 1) akf = false;
   if (sb0 == 1 && sb1 != 1) bnf = false;

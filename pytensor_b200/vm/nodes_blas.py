@@ -271,14 +271,8 @@ class GemmNode(Node):
             out = dev.empty((M, N), self.dtype)
             if out.numel() and beta != 0.0:
                 dev.copy_strided(out, _broadcast_view(Z, (M, N)))
-        if out.numel():
-            if X.shape[1] == 0:
-                if beta == 0.0:
-                    _zero_fill(out)
-                else:
-                    gemm(self.dtype, 0.0, out[:, :1], out[:1, :], beta, out, 0)
-            else:
-                gemm(self.dtype, alpha, X, Y, beta, out, self.precision, b_key=y.key)
+        if out.numel():   # (an empty contraction gives alpha * 0 + beta * z: the FMA kernel's k-loop does not run)
+            gemm(self.dtype, alpha, X, Y, beta, out, self.precision, b_key=y.key)
         return [Val(d=out)]
 
 
@@ -294,14 +288,7 @@ class GemvNode(Node):
         Y, Am, X = y.dev(), A.dev(), x.dev()
         al, be = _scalar(alpha), _scalar(beta)
         out = Y if self.inplace else (dev.clone(Y) if be != 0.0 else dev.empty(tuple(Y.shape), self.dtype))
-        if out.numel():
-            if Am.shape[1] == 0:
-                al = 0.0
-                Am = out.as_strided((out.shape[0], 1), (out.stride(0), 1), out.storage_offset())
-                X = out[:1]
-                if be == 0.0:
-                    _zero_fill(out)
-                    return [Val(d=out)]
+        if out.numel():   # (an empty contraction gives alpha * 0 + beta * y: the row kernel's loop does not run)
             gemv(self.dtype, al, Am, X, be, out)
         return [Val(d=out)]
 
@@ -381,9 +368,7 @@ class GemmBiasActNode(Node):
                 raise ValueError(f"{self.name}: bias of shape {tuple(bias.shape)} does not match N={N}")
             b1 = bias.reshape(-1) if bias.is_contiguous() else dev.contiguous(bias).reshape(-1)
         out = dev.empty((M, N), self.dtype)
-        if out.numel():
-            if A.shape[1] == 0:
-                raise NotImplementedError("fused bias epilogue with K == 0")
+        if out.numel():   # (K == 0: the FMA kernel writes act(0 + bias))
             aux = gemm(self.dtype, 1.0, A, B, 0.0, out, self.precision, bias=b1, act=self.act, a_staged=vals[0].aux,
                        want_staged=self.emit_bf16, b_key=vals[1].key)
             return [Val(d=out, aux=aux)]

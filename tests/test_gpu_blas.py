@@ -112,6 +112,20 @@ def test_gemm_zero_sized_and_broadcast_z(gpu):
     compare_cuda_and_cvm([x, y], [pt.dot(x, y)], [rng.standard_normal((4, 0)), np.zeros((0, 7))])
     compare_cuda_and_cvm([zrow, x, y], [zrow + 2.0 * pt.dot(x, y)],
                          [rng.standard_normal((1, 7)), rng.standard_normal((4, 5)), rng.standard_normal((5, 7))])
+    # an empty contraction leaves b * z (gemm.py: z *= b; z += a * dot): inf, NaN and values whose products overflow stay
+    # in their own elements, in Gemm and in Gemv
+    for dtype, huge in (("float64", 1e200), ("float32", 1e20)):
+        z, a, b = pt.matrix("z", dtype=dtype), pt.matrix("a", dtype=dtype), pt.matrix("b", dtype=dtype)
+        yv, A, v = pt.vector("yv", dtype=dtype), pt.matrix("A", dtype=dtype), pt.vector("v", dtype=dtype)
+        zv = rng.standard_normal((4, 7)).astype(dtype)
+        zv[0, 0], zv[1, 2], zv[2, 3], zv[3, :], zv[:, 6] = np.inf, np.nan, -np.inf, huge, huge
+        yvv = rng.standard_normal(6).astype(dtype)
+        yvv[0], yvv[2], yvv[4] = np.inf, np.nan, huge
+        f, _ = compare_cuda_and_cvm([z, a, b, yv, A, v], [0.5 * z + 2.0 * pt.dot(a, b), 0.5 * yv + 2.0 * pt.dot(A, v)],
+                                    [zv, np.zeros((4, 0), dtype), np.zeros((0, 7), dtype), yvv, np.zeros((6, 0), dtype),
+                                     np.zeros(0, dtype)])
+        names = [type(n.op).__name__ for n in f.maker.fgraph.toposort()]
+        assert "Gemm" in names and "Gemv" in names, names
 
 
 def test_gemv_beta_zero_ignores_nan_y(gpu):

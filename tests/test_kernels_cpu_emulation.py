@@ -738,6 +738,7 @@ def _blas_text():
     ("float32", False, True, 64, 64, 16, 0.6, False, 0),      # A transposed view (M fast), exact tiles, beta * C
     ("float64", True, False, 33, 47, 29, -1.0, False, 0),     # B transposed view (K fast)
     ("float64", False, False, 5, 200, 3, 1.0, True, 0),       # both transposed, K smaller than one k-tile
+    ("float32", True, False, 300, 70, 20, -0.5, True, 0),     # 5 m-tiles on 2 y-blocks: the grid-stride m-tile loop turns
 ])
 def test_fma_gemm_kernel_strides_edges_and_epilogue(tmp_path, dtype, a_kfast, b_nfast, M, N, K, beta, with_bias, act):
     """C = act(alpha*A@B + beta*C + bias) over arbitrary element strides; beta == 0 never reads C (NaN-poisoned here, the
@@ -769,7 +770,7 @@ def test_fma_gemm_kernel_strides_edges_and_epilogue(tmp_path, dtype, a_kfast, b_
             c_longlong(B.strides[1] // isz), ct(beta), c_void_p(C.ctypes.data), c_longlong(C.strides[0] // isz),
             c_longlong(C.strides[1] // isz), _ptr(bias) if with_bias else c_void_p(None), c_int(act)]
     untouched = Cbuf[:, 1::2].copy()
-    k.launch(((N + 63) // 64, (M + 63) // 64), 256, args)
+    k.launch(((N + 63) // 64, min((M + 63) // 64, 2)), 256, args)   # (fewer y-blocks than m-tiles where M > 128)
     tol = 2e-5 if dtype == "float32" else 1e-12
     np.testing.assert_allclose(C, expect, rtol=tol, atol=tol)
     np.testing.assert_array_equal(Cbuf[:, 1::2], untouched)   # the columns between the strided ones are not written
